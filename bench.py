@@ -65,7 +65,7 @@ def workload_of(args):
 
 
 def config_block(infer, workload, world):
-    """Identical for both arms (the driver compares the dicts): what is computed, not how."""
+    """Identical for both arms (so that their result lines can be compared): what is computed, not how."""
     return {"workload": workload, "ddim_steps": infer["inference_steps"], "guided_steps": infer["guidance_steps"],
             "video_length": infer["video_length"], "replicas": world,
             "l2": "inputs larger than L2 (2.6 GB of weights stream through every UNet forward)"}
@@ -76,7 +76,7 @@ def log(*a):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (a power- or heat-throttled run is visible)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -243,7 +243,7 @@ def run_reference_arm(args):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# same-GPU comparator (BASELINE.md §4 "B-GPU-ref"): the reference's op sequence in fp16 on this B200
+# same-GPU comparator (BASELINE.md §4 "B-GPU-ref"): the reference's op sequence in fp16 on the same GPU
 # ----------------------------------------------------------------------------------------------------------------
 def gpu_reference_steps(infer: dict, dev, reps: int = 2):
     """The oracle port = the reference's own op sequence (per-frame rearranges, separate q/k/v projections, text
@@ -288,15 +288,6 @@ def gpu_reference_steps(infer: dict, dev, reps: int = 2):
 # ----------------------------------------------------------------------------------------------------------------
 # this package's arm
 # ----------------------------------------------------------------------------------------------------------------
-def _ncu_traffic():
-    """Per-launch DRAM traffic of the roofline kernel from the committed ncu capture (profiles/r02_temporal_traffic.json,
-    written by scripts/summarize_traffic.py from `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum`)."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r02_temporal_traffic.json")))
-    except Exception:
-        return None
-
-
 def run_own_arm(args):
     import motionclone_b200 as mc
     from motionclone_b200 import _lib, dist as mcdist, guidance, ops
@@ -383,9 +374,11 @@ def run_own_arm(args):
             tdist.all_reduce(ms, op=tdist.ReduceOp.MAX)
         return ms.item()
 
+    last_out = {}
+
     def step_resident(i):
         pipe.set_prompt_embeds(text_res[i])
-        pipe.sample_video(noisy_latents=resident[i], return_latents=True, add_controlnet=use_cn)
+        last_out["latents"] = pipe.sample_video(noisy_latents=resident[i], return_latents=True, add_controlnet=use_cn)
 
     out_host = torch.empty(1, 4, L, infer["height"] // 8, infer["width"] // 8, dtype=torch.float16).pin_memory()
 
@@ -405,6 +398,8 @@ def run_own_arm(args):
     _lib.reset_launch_count()
     ms = timed(step_resident, args.steps, args.warmup)
     launches = _lib.launch_count()
+    if args.dump_outputs and rank == 0:  # what the last timed step returned, before any later step can overwrite it
+        dump_outputs(args.dump_outputs, last_out)
     ms_e2e = timed(step_e2e, args.steps, args.warmup + args.steps)
     clk = clocks.finish()
     # roofline leg: ONE more sample with a CUDA-event pair around every launch of this package's attention kernels (on the
@@ -427,20 +422,16 @@ def run_own_arm(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    tpeak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))                 # H100 SXM data sheet: 3.35 TB/s HBM3
+    tpeak = float(peaks.get("bf16_tflops_sustained", 989.0))   # H100 SXM data sheet: 989 TFLOP/s dense fp16 / bf16
     n_l, n_b, n_ms = ksum.get("temporal_attn_fwd", (0, 0, 0.0))
     achieved = (n_b / 1e9) / (n_ms / 1e3) if n_ms > 0 else None
-    traffic = _ncu_traffic()
     roof = {"kernel": "temporal_attn_fwd_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
             "frac": (achieved / peak) if achieved else None,
-            "traffic": traffic["dram_bytes_per_launch"] if traffic else None,
-            "traffic_source": traffic["source"] if traffic else "no committed ncu dram capture",
-            "peak_source": "MEASURED_PEAKS.json (burst copy)" if peaks else "fallback 6.65 TB/s (B200_PROFILING.md)",
+            "peak_source": "MEASURED_PEAKS.json (burst copy)" if peaks else "H100 SXM data sheet (3.35 TB/s, 989 TFLOP/s at 700 W)",
             "launches": n_l, "algorithmic_bytes_per_launch": (n_b / n_l) if n_l else None,
             "avg_launch_us": (1e3 * n_ms / n_l) if n_l else None,
-            "l2_policy": "in situ: Q/K/V were just written by the QKV GEMM and can be L2-resident; "
-                         "profiles/ holds the cold-L2 per-shape numbers"}
+            "l2_policy": "in situ: Q/K/V were just written by the QKV GEMM and can be L2-resident"}
     b_l, b_b, b_ms = ksum.get("temporal_attn_bwd", (0, 0, 0.0))
     if b_ms > 0:
         roof["bwd"] = {"launches": b_l, "achieved": (b_b / 1e9) / (b_ms / 1e3), "frac": (b_b / 1e9) / (b_ms / 1e3) / peak}
@@ -476,7 +467,7 @@ def run_own_arm(args):
     lat_bytes = host[0].numel() * 2
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f16", "data": "synthetic",
+            "dtype": "f16", "data": "synthetic", "device": torch.cuda.get_device_name(dev),
             "config": config_block(infer, workload, world),
             "arm": f"replica x{world} (independent samples), one NCCL broadcast of the motion representation; "
                    f"cuda graphs {'on' if pipe.use_cuda_graphs else 'off'}",
@@ -486,6 +477,15 @@ def run_own_arm(args):
                     "d2h_bytes_per_step": lat_bytes, "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": int(launches), "clocks": clk, "roofline": roof, "gpu_reference": gpu_ref, "cpu_baseline": cpu}
     _emit(line)
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Each array as DIR/<name>.npy in float32. The inputs are seeded, so two builds given the same arguments can be
+    compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 _RESULT_FD = None
@@ -507,14 +507,18 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="object", choices=list(CONFIGS),
-                    help="BASELINE.json configs[1..4]; `object` (configs[1]) is the headline the driver runs")
+                    help="BASELINE.json configs[1..4]; `object` (configs[1]) is the headline workload")
     ap.add_argument("--ddim-steps", type=int, default=50, help="profiling only: anything but 50 is not a bench value")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-cuda-graphs", action="store_true", help="A/B: launch the no-grad UNet forwards eagerly")
     ap.add_argument("--ref-budget", type=float, default=240.0, help="seconds of CPU work for --impl reference")
     ap.add_argument("--cpu-budget", type=float, default=60.0, help="seconds of CPU work for the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final latents of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs needs --impl ours: the reference arm times a bounded CPU sample, not the full denoising loop")
     # The contract is ONE JSON line on stdout. Libraries write there too (NCCL prints its version banner on the first
     # communicator when NCCL_DEBUG=VERSION is set in the environment), so everything but the result goes to stderr: file
     # descriptor 1 is pointed at stderr for the run and the line is written to the saved descriptor at the end.

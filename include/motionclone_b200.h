@@ -1,5 +1,5 @@
 /*
- * motionclone_b200 — C ABI of the B200 (sm_100a) kernels behind MotionClone's guided denoising path.
+ * motionclone_b200 — C ABI of the H100 (sm_90a) kernels behind MotionClone's guided denoising path.
  *
  * The reference (LPengYang/MotionClone) has no FFI: its "operator API" is a Python method surface executed by ATen /
  * cuBLAS / xformers kernels (SURVEY.md §8b). These entry points are what a binding for that surface calls; each one
@@ -114,7 +114,7 @@ int mc_add_noise(const void* x0, const void* noise, void* out, int64_t n, float 
                  void* stream);
 
 /*
- * Text cross-attention forward on tcgen05 tensor cores with TMEM accumulators (csrc/cross_attn_fwd_tc.cu):
+ * Text cross-attention forward on wgmma tensor cores (csrc/spatial_attn_tc.cu, the spatial forward's kernel):
  * O = softmax(scale * Q K^T) V per (batch, head), Q [B, Nq, H*DH] (all frames of one prompt), K, V [B, Nk <= 80, H*DH].
  * Replaces the xformers call for `attn2` (models/attention.py:193-201, :280-285 -> :535-542).
  * Strides in elements (multiples of 8); head h occupies columns [h*DH, (h+1)*DH). DH in {16, 32, 40, 64, 80, 160}.
@@ -124,7 +124,7 @@ int mc_cross_attn_fwd(const void* q, const void* k, const void* v, void* o, int 
                       int64_t o_stride_b, int64_t o_stride_row, float scale, void* stream);
 
 /*
- * Gradient of the same cross-attention with respect to Q only (tcgen05, csrc/cross_attn_bwd_tc.cu):
+ * Gradient of the same cross-attention with respect to Q only (wgmma, csrc/spatial_attn_bwd_tc.cu):
  * dQ = scale * [P o (dO V^T - rowsum(P o dO V^T))] K with P recomputed from Q, K. The text K / V are projections of a
  * constant prompt embedding through frozen weights (t2v_video_sample.py:67-68), so torch.autograd.grad w.r.t. the
  * latents (utils/motionclone_functions.py:236) never asks for dK / dV; the Python wrapper raises if it is asked to.
@@ -136,9 +136,9 @@ int mc_cross_attn_bwd_dq(const void* q, const void* k, const void* v, const void
                          int64_t dq_stride_row, float scale, void* stream);
 
 /*
- * Spatial self-attention on tcgen05 tensor cores with TMEM accumulators and tensor-map TMA operand loads
+ * Spatial self-attention on wgmma tensor cores (register accumulators) with tensor-map TMA operand loads
  * (csrc/spatial_attn_tc.cu): O = softmax(scale * Q K^T) V per (frame, head) over the N tokens of one frame, any N >= 1
- * (128-key tiles, online softmax). Replaces the xformers call for `attn1`
+ * (64-key tiles, online softmax). Replaces the xformers call for `attn1`
  * (models/attention.py:190-192, :271-278 -> :535-542, xformers.ops.memory_efficient_attention, attn_bias=None).
  * q, k, v, o: [B, N, H*DH] views with their own frame / token strides in elements (multiples of 8; 16-byte aligned
  * pointers), head h in columns [h*DH, (h+1)*DH) - e.g. the column blocks of one fused QKV projection.
@@ -154,8 +154,8 @@ int mc_spatial_attn_fwd(const void* q, const void* k, const void* v, void* o, fl
  * Backward of mc_spatial_attn_fwd w.r.t. q, k, v (the autograd of the xformers seam that torch.autograd.grad traverses,
  * utils/motionclone_functions.py:236): dV = P^T dO, dS = scale * P o (dO V^T - rowsum(dO o O)), dQ = dS K, dK = dS^T Q,
  * with P recomputed from the forward's log-sum-exp `lse` [B, H, N]. Three launches: rowsum(dO o O) -> workspace, a dQ
- * kernel (128-query CTAs streaming 64-key tiles) and a dK/dV kernel (128-key CTAs streaming 64-query tiles); tcgen05 +
- * TMEM + tensor-map TMA throughout, no atomics (deterministic). o, d_o: [B, N, H*DH] with their own strides; dq, dk, dv
+ * kernel (128-query CTAs streaming 64-key tiles) and a dK/dV kernel (128-key CTAs streaming 64-query tiles); wgmma +
+ * tensor-map TMA throughout, no atomics (deterministic). o, d_o: [B, N, H*DH] with their own strides; dq, dk, dv
  * share g_stride_* (e.g. the column blocks of one fused [B, N, 3*H*DH] gradient buffer).
  * workspace: mc_spatial_attn_bwd_workspace_bytes(B, N, H) bytes of device memory (fp32 [B, H, N]).
  */

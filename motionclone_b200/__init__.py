@@ -1,4 +1,4 @@
-"""motionclone_b200 — B200-native (sm_100a) implementation of MotionClone's guided video-diffusion denoising loop,
+"""motionclone_b200 — H100-native (sm_90a) implementation of MotionClone's guided video-diffusion denoising loop,
 behind the reference's own Python surface (VersatileAttention / CrossAttention / the nine bound functions).
 See DESIGN.md; the C ABI underneath is include/motionclone_b200.h."""
 from . import _lib  # noqa: F401

@@ -7,8 +7,8 @@ import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_uint8, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# The one library this package loads. (A/B scripts under scripts/ point this attribute at a side-by-side build of the same
-# sources BEFORE the first call - scripts/build_variant.sh; nothing in the package or in the environment selects a library.)
+# The one library this package loads (A/B scripts may point this attribute at a side-by-side build of the same sources
+# BEFORE the first call; nothing in the package or in the environment selects a library).
 LIB_PATH = os.path.join(_HERE, "libmotionclone_b200.so")
 
 
@@ -37,7 +37,7 @@ def lib() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise MotionCloneKernelError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). motionclone_b200 has no CPU or eager fallback.")
+            "(nvcc, sm_90a). motionclone_b200 has no CPU or eager fallback.")
     L = ctypes.CDLL(LIB_PATH)
     P = c_void_p
     L.mc_abi_version.restype = c_int

@@ -1,4 +1,4 @@
-// Fused elementwise / reduction kernels of the guided step (sm_100a): CFG combine + score-guided DDIM update,
+// Fused elementwise / reduction kernels of the guided step (sm_90a): CFG combine + score-guided DDIM update,
 // add_noise, stand-alone top-1, and the motion-guidance loss with its closed-form gradient.
 // All are HBM / launch-latency bound: 128-bit coalesced accesses, grid sized in multiples of the SM count.
 #include <mutex>
@@ -7,7 +7,7 @@
 
 namespace mc {
 
-constexpr int kSMs = 148;
+constexpr int kSMs = 132;  // H100 SXM
 
 union Pack8 {
   uint4 u;

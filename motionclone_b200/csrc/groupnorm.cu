@@ -1,12 +1,12 @@
 // GroupNorm(32) [+ time-embedding add] [+ SiLU] on channels_last `[(b f), h, w, C]` fp16 activations, forward and input
-// gradient (sm_100a). Reference: InflatedGroupNorm + nonlinearity, models/resnet.py:21-29, :186-204; the transformer
+// gradient (sm_90a). Reference: InflatedGroupNorm + nonlinearity, models/resnet.py:21-29, :186-204; the transformer
 // input norms models/attention.py:61,105 and models/motion_module.py:112,145 — all through ATen's NCHW GroupNorm, which
 // on a channels_last activation costs a layout copy in, a layout copy before the next cuDNN conv and two passes of
 // its own. These kernels read NHWC directly.
 //
 // HBM-bound: forward = 2 reads + 1 write of the tensor (statistics pass, then apply; the second read is an L2 hit for
-// tensors under ~60 MB), backward = 2 x (x, dz) reads + 1 write. What bounds a streaming kernel on B200 is bytes in
-// flight per SM, and register-staged loads cap that at 40-60 KB (measured: 26-40 % of the HBM roof, profiles/README.md).
+// tensors under ~60 MB), backward = 2 x (x, dz) reads + 1 write. What bounds a streaming kernel is bytes in flight per
+// SM, and register-staged loads cap that at 40-60 KB.
 // So the tensor moves like the temporal-attention tiles do:
 //   * a CTA owns a CONTIGUOUS run of pixels of one frame and walks it in tiles of <= 32 KB, each brought in by ONE bulk
 //     copy (cp.async.bulk, TMA engine, SASS UBLKCP) signalled on an mbarrier, two stages deep: tile t+1 is in flight
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(512, 2) groupnorm_stats_kernel(const __half* _
     gn_fetch(buf + (t & 1) * stage_bytes, x, n, HW, C, p0, npx, bar + (t & 1));
   };
   if (tid == 0 && ntrips > 0) fetch(0);
-  uint64_t sum2[4], sq2[4];  // channel pairs (2j, 2j + 1): FADD2 / FFMA2, bit-identical to eight scalar accumulators
+  uint64_t sum2[4], sq2[4];  // channel pairs (2j, 2j + 1): eight fp32 accumulators
 #pragma unroll
   for (int j = 0; j < 4; ++j) sum2[j] = sq2[j] = f2_pack(0.f, 0.f);
   const bool has_cb = chan_bias != nullptr;
@@ -531,7 +531,7 @@ struct GnTiling {
 };
 
 // `tensors` tiles of <= tile_bytes each per stage, two stages (64 KB per CTA -> 3 CTAs per SM; the backward kernels hold
-// more registers: 2). ONE wave: at most 148 x ctas_per_sm CTAs in the grid, each walking ceil(tiles / S) tiles through its two-stage pipeline (a grid of 1.5 waves costs
+// more registers: 2). ONE wave: at most 132 x ctas_per_sm CTAs in the grid, each walking ceil(tiles / S) tiles through its two-stage pipeline (a grid of 1.5 waves costs
 // two: measured on the 16 x 64 x 64 x 320 layers).
 static GnTiling gn_tiling(int N, int HW, int C, int NT, int tensors, int tile_bytes, int ctas_per_sm) {
   GnTiling t;
@@ -539,7 +539,7 @@ static GnTiling gn_tiling(int N, int HW, int C, int NT, int tensors, int tile_by
   if (t.PX < 1) t.PX = 1;
   if (t.PX > HW) t.PX = HW;
   const int tiles = (HW + t.PX - 1) / t.PX;
-  t.S = (148 * ctas_per_sm) / N;
+  t.S = (132 * ctas_per_sm) / N;
   if (t.S < 1) t.S = 1;
   if (t.S > tiles) t.S = tiles;
   if (t.S > kGnMaxSplits) t.S = kGnMaxSplits;

@@ -1,4 +1,4 @@
-// Shared device helpers (sm_100a): mbarrier + bulk-copy (TMA 1-D, UBLKCP) staging, ldmatrix / mma.sync fragments.
+// Shared device helpers (sm_90a): mbarrier + bulk-copy (TMA 1-D, UBLKCP) staging, ldmatrix / mma.sync fragments.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -36,8 +36,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 
 // try_wait with a suspend-time hint: the thread sleeps in hardware until the phase completes (or the hint, ~10 ms, expires)
-// instead of re-issuing the probe - waiting warps then leave the issue slots to the warps that compute (round-2 ncu of the
-// attention kernels: 22-28 % of the executed instructions were BRA / SYNCS / YIELD of spin loops without the hint)
+// instead of re-issuing the probe - waiting warps then leave the issue slots to the warps that compute
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -76,26 +75,22 @@ __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bu
 // generic-proxy smem writes -> visible to the async proxy (bulk store engine)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- packed fp32 pairs (sm_100: FADD2 / FFMA2 issue two IEEE fp32 operations per lane and instruction) ----
-// Each half of a pair is an ordinary round-to-nearest fp32 operation: results are bit-identical to the scalar code, the
-// issue count halves (the GroupNorm statistics pass is bound by instruction issue, not by HBM).
+// ---- fp32 pairs carried in one 64-bit value: each half is an ordinary round-to-nearest fp32 operation ----
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t v;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(v) : "f"(lo), "f"(hi));
-  return v;
+  return (uint64_t)__float_as_uint(lo) | ((uint64_t)__float_as_uint(hi) << 32);
 }
 __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = __uint_as_float((uint32_t)v), hi = __uint_as_float((uint32_t)(v >> 32));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1), f2_unpack(b, b0, b1);
+  return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1), f2_unpack(b, b0, b1), f2_unpack(c, c0, c1);
+  return f2_pack(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
 // ---- ldmatrix ----

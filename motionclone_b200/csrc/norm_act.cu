@@ -1,4 +1,4 @@
-// Memory-bound glue of the UNet3D forward and of the guided pass's backward on token-major fp16 activations (sm_100a):
+// Memory-bound glue of the UNet3D forward and of the guided pass's backward on token-major fp16 activations (sm_90a):
 //   * LayerNorm over C (+ the temporal positional-encoding add)    (models/attention.py:189-212, motion_module.py:204-215,
 //     :281-282), forward and input gradient
 //   * GEGLU  h * gelu_erf(gate), forward and backward               (diffusers-0.16 FeedForward used at attention.py:211,
@@ -257,7 +257,7 @@ extern "C" int mc_layernorm(const void* x, void* y, const void* gamma, const voi
   const size_t smem = 2 * (size_t)TR * C * 2 + 16 + 3 * (size_t)C * 2;
   int per_sm = (int)((227 * 1024) / (smem + 1024));
   per_sm = per_sm > 8 ? 8 : per_sm;
-  int64_t blocks = n_tiles < (int64_t)148 * per_sm ? n_tiles : (int64_t)148 * per_sm;
+  int64_t blocks = n_tiles < (int64_t)132 * per_sm ? n_tiles : (int64_t)132 * per_sm;
   cudaStream_t st = (cudaStream_t)stream;
   const int vpl = (C / 8 + 31) / 32;
 #define MC_LN(V)                                                                                                   \
@@ -295,7 +295,7 @@ extern "C" int mc_geglu(const void* in, void* out, int64_t T, int I, void* strea
   }
   const int64_t nvec = T * (I / 8);
   cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (nvec >= (int64_t)1 << 20 && cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev < 64) {
     // >= 16 MB of output: the persistent table kernel (one 1024-thread CTA per SM, 128 KB of shared memory)
     if (!g_gelu_lut_ready[dev]) {  // once per device, ordered before the first use on this stream
@@ -312,7 +312,7 @@ extern "C" int mc_geglu(const void* in, void* out, int64_t T, int I, void* strea
     return check_launch("geglu_lut");
   }
   int64_t blocks = (nvec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   geglu_kernel<<<(unsigned)blocks, 256, 0, st>>>((const __half*)in, (__half*)out, T, I);
   count_launch();
   return check_launch("geglu");
@@ -453,7 +453,7 @@ extern "C" int mc_layernorm_bwd(const void* x, const void* dy, void* dx, const v
     return MC_E_UNSUPPORTED;
   }
   int64_t blocks = (rows + 7) / 8;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   cudaStream_t st = (cudaStream_t)stream;
   const int vpl = (C / 8 + 31) / 32;
 #define MC_LNB(V)                                                                                                     \
@@ -483,7 +483,7 @@ extern "C" int mc_geglu_bwd(const void* in, const void* dout, void* din, int64_t
   }
   const int64_t nvec = T * (I / 8);
   int64_t blocks = (nvec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   geglu_bwd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)in, (const __half*)dout, (__half*)din,
                                                                         T, I);
   count_launch();

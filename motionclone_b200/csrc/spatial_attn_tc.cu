@@ -1,363 +1,214 @@
-// Spatial self-attention (S1) on 5th-gen tensor cores: tcgen05.mma with TMEM accumulators, operands staged by tensor-map
-// TMA (cp.async.bulk.tensor), sm_100a. Forward (this file); the backward (dQ kernel, dK/dV kernel) is csrc/spatial_attn_bwd_tc.cu.
+// Attention forward on Hopper tensor cores (wgmma with register accumulators), operands staged by tensor-map TMA
+// (cp.async.bulk.tensor), sm_90a. Serves two seams of the reference:
+//   * spatial self-attention `attn1` (models/attention.py:190-192, :271-278 -> :535-542,
+//     xformers.ops.memory_efficient_attention(q, k, v, attn_bias=None)): O = softmax(scale Q K^T) V per (frame, head)
+//     over the N = h*w tokens of one frame; N = 4096 / 1024 / 256 / 64 and DH = 40 / 80 / 160 / 160 at 16 x 512 x 512;
+//     the natural-log sum-exp of every query row is kept for the backward (csrc/spatial_attn_bwd_tc.cu);
+//   * text cross-attention `attn2` (models/attention.py:193-201, :280-285): Q [b, f*N, C] (all frames of one prompt)
+//     against the 77 text tokens K / V [b, 77, C].
+// fp32 softmax statistics, one rounding of the output (xformers / flash semantics - SURVEY.md appendix "Attention
+// numerics").
 //
-// Replaces the xformers seam of `attn1` (reference models/attention.py:190-192, :271-278 -> :535-542,
-// xformers.ops.memory_efficient_attention(q, k, v, attn_bias=None)): O = softmax(scale Q K^T) V per (frame, head) over the
-// N = h*w tokens of one frame; N = 4096 / 1024 / 256 / 64 and DH = 40 / 80 / 160 / 160 at 16 x 512 x 512. fp32 softmax
-// statistics, one rounding of the output (xformers / flash semantics - SURVEY.md appendix "Attention numerics").
-//
-// Forward, one CTA = one (frame, head, 128-query tile); 192 threads = 4 softmax warps (thread r owns query row r = TMEM
-// lane r) + 1 MMA warp (lane 0 issues every tcgen05.mma) + 1 load warp (lane 0 issues every TMA load). Key tiles of 64;
-// the score tile S is DOUBLE-BUFFERED in tensor memory so that the tensor pipe computes S_{j+1} while the softmax warps
-// are still working on S_j (S_{j+1} = Q K_{j+1}^T does not depend on them):
-//   MMA warp:  S_{j+1} = Q K_{j+1}^T   tcgen05.mma M=128 N=64 K=DH, A/B from shared memory -> TMEM buffer (j+1)&1  -> commit s_full[(j+1)&1]
-//   softmax :  S_j -> registers (64 fp32 per thread), row max, exp2, P_j -> fp16 pairs -> tcgen05.st back over the first 32
-//              columns of the thread's own lane in buffer j&1 (its own, already consumed, S_j)                    -> arrive p_full[j&1]
-//   MMA warp:  O += P_j V_j            tcgen05.mma with the A operand (P) read FROM TENSOR MEMORY, B = V_j MN-major straight
-//              from its TMA tile (no transpose)                                           -> commit pv_done, stage_free[j % NS]
-// Pipe order S0 S1 PV0 S2 PV1 S3 ...: the tensor pipe executes in issue order, so S_{j+2} (which overwrites buffer j&1) is
-// behind P V_j (which reads P_j from it). Round-2 ncu of the single-buffered version: the softmax warps spent 35 % of their
-// time parked on s_full - S_{j+1} could only be issued behind P V_j, i.e. after the slowest of the four warps had finished
-// tile j - and moving half of the exponentials to the FMA pipe changed nothing: the kernel was bound by that serial
-// chain, not by MUFU throughput.
-// P never touches shared memory: the only shared-memory traffic is TMA writes and the MMA's operand reads. O stays in TMEM
-// for the whole key loop; the running maximum is only raised when a row's maximum grows by more than 2^8 (P <= 256 fits
-// fp16; exactness is unaffected because numerator and denominator share the reference maximum); only then does the softmax
-// warp rescale its 32 rows of O (tcgen05.ld -> multiply -> tcgen05.st). K and V tiles stream through an NS-stage TMA ring.
+// One CTA = one (frame or batch, head, 128-query tile); 288 threads = 2 consumer warpgroups (64 query rows each) + 1
+// producer warp whose lane 0 issues every TMA load. The Q tile is loaded once; K and V tiles of 64 keys stream through an
+// NS-stage ring (full barriers: TMA transaction bytes; empty barriers: one arrival per consumer warp). Per key tile j a
+// consumer warpgroup computes
+//   S = Q K_j^T      wgmma m64n64k16, A = its 64 Q rows and B = K_j, both K-major from shared memory
+//   online softmax   row max / sum across the 4 threads of a row quad, O rescaled in registers, P -> fp16 A fragments
+//   O += P V_j       wgmma m64nWk16 with A = P from registers, B = V_j read MN-major straight from its TMA tile
+// Keys past the end of the sequence are zero-filled by the TMA unit and masked to -inf in S.
 #include <math.h>
 
 #include "tma_common.cuh"
 
 namespace mc {
 
-constexpr int kFM = 128;         // query rows per CTA (UMMA M)
-constexpr int kFBN = 64;         // keys per tile (UMMA N of S, K extent of P V)
-constexpr int kFThreads = 192;   // 4 softmax warps + MMA warp + load warp
-constexpr int kFMmaWarp = 4, kFTmaWarp = 5;
-constexpr float kRescaleThreshold = 8.f;  // log2 units
+constexpr int kFM = 128;                    // query rows per CTA
+constexpr int kFBN = 64;                    // keys per tile
+constexpr int kFWG = kFM / 64;              // consumer warpgroups
+constexpr int kFThreads = kFWG * 128 + 32;  // + producer warp
+constexpr int kFProducerWarp = kFWG * 4;
 
 struct FAParams {
-  float* lse;        // [B][H][N] natural-log sum-exp of the scaled scores (nullable)
+  float* lse;        // [B][H][Nq] natural-log sum-exp of the scaled scores (nullable)
   __half* o;
   int64_t o_sb, o_sr;
-  int B, N, H;
+  int B, Nq, Nk, H;
   float scale_log2e;  // scale * log2(e)
 };
 
 template <int DH>
 struct FACfg {
-  using T = TileParts<DH>;            // Q tile (128 rows)
-  static constexpr int DHP = T::DHP;
-  static constexpr int BN = kFBN;
-  using TK = TileParts<DH, BN>;       // K / V tiles
-  // Row sums: when the head dim leaves zero-padded columns in the V tile (DH = 40 -> 48), column DH of V is set to 1.0
-  // after every TMA load, so accumulator column DH of O = P V IS the row sum (from the same fp16 P as the numerator, at no
-  // extra MMA and no extra instruction in the softmax warps). Otherwise the softmax threads add their probabilities.
-  static constexpr bool PAD_SUM = DHP > DH && DH < 64;
-  static constexpr int NS = DHP <= 80 ? 4 : 3;               // K / V ring depth
-  static constexpr int OFF_Q = 0, OFF_K = T::BYTES, OFF_V = OFF_K + NS * TK::BYTES;
-  static constexpr int OFF_BAR = OFF_V + NS * TK::BYTES;
-  static constexpr int SMEM = OFF_BAR + 256 + 1024;          // + alignment slack (dynamic smem base is 16 B aligned)
-  static constexpr int O_COL = 2 * BN;                       // S / P buffers at TMEM [0, BN), [BN, 2 BN); O at [2 BN, 2 BN + DHP)
-  static constexpr int ACC_COLS = DHP;
-  static constexpr int TCOLS = (O_COL + ACC_COLS <= 256) ? 256 : 512;
-  static constexpr int CTAS_TMEM = 512 / TCOLS, CTAS_SMEM = (227 * 1024) / SMEM;
-  static constexpr int CTAS_PER_SM = CTAS_TMEM < CTAS_SMEM ? CTAS_TMEM : (CTAS_SMEM < 1 ? 1 : CTAS_SMEM);
+  using TQ = TileParts<DH, kFM>;
+  using TK = TileParts<DH, kFBN>;
+  static constexpr int ACC = AccW<DH>::REGS;       // O accumulator registers per thread
+  static constexpr int NS = DH <= 80 ? 4 : 3;      // K / V ring depth
+  static constexpr int QB = align1k(TQ::BYTES), KB = align1k(TK::BYTES);
+  static constexpr int OFF_Q = 0, OFF_K = QB, OFF_V = OFF_K + NS * KB, OFF_BAR = OFF_V + NS * KB;
+  static constexpr int SMEM = OFF_BAR + 256 + 1024;  // + alignment slack (dynamic smem base is 16 B aligned)
 };
 
-// S tile: A = Q (K-major, 128 rows), B = K (K-major, BN rows); one MMA per k16 step over the head dim
 template <int DH>
-__device__ __forceinline__ void issue_qk(uint32_t d_tmem, uint32_t sA, uint32_t sB) {
-  using T = TileParts<DH>;
-  using TK = typename FACfg<DH>::TK;
-  const uint32_t idesc = umma_idesc_f16(kFM, FACfg<DH>::BN, false, false);
-  uint32_t acc = 0;
-#pragma unroll
-  for (int p = 0; p < T::N64; ++p)
-#pragma unroll
-    for (int ks = 0; ks < T::KS64; ++ks) {
-      umma_f16(d_tmem, desc_k128(sA + T::part64_off(p), ks), desc_k128(sB + TK::part64_off(p), ks), idesc, acc);
-      acc = 1;
-    }
-#pragma unroll
-  for (int p = 0; p < T::N16; ++p) {
-    umma_f16(d_tmem, desc_k32(sA + T::part16_off(p)), desc_k32(sB + TK::part16_off(p)), idesc, acc);
-    acc = 1;
-  }
-}
-
-// O[128 x DH] (+)= P[128 x BN] V[BN x DH]: A = P in tensor memory (8 packed columns per k16 step), B = the V tile read
-// MN-major (its rows are the K dimension). One MMA per (k16 step, part of B).
-template <int DH>
-__device__ __forceinline__ void issue_pv(uint32_t o_tmem, uint32_t p_tmem, uint32_t sB, bool accumulate) {
+__global__ void __launch_bounds__(kFThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap mq128, const __grid_constant__ CUtensorMap mk128,
+                const __grid_constant__ CUtensorMap mv128, const __grid_constant__ CUtensorMap mq32,
+                const __grid_constant__ CUtensorMap mk32, const __grid_constant__ CUtensorMap mv32, const FAParams prm) {
   using X = FACfg<DH>;
-  using T = typename X::TK;
-  const uint32_t idesc64 = umma_idesc_f16(kFM, T::W64, false, true);
-  const uint32_t idesc16 = umma_idesc_f16(kFM, 16, false, true);
-#pragma unroll
-  for (int ks = 0; ks < X::BN / 16; ++ks) {
-    const uint32_t a = p_tmem + ks * 8;
-    const uint32_t acc = (accumulate || ks > 0) ? 1u : 0u;
-#pragma unroll
-    for (int p = 0; p < T::N64; ++p) umma_f16_ts(o_tmem + p * 64, a, desc_mn128(sB + T::part64_off(p), ks), idesc64, acc);
-#pragma unroll
-    for (int p = 0; p < T::N16; ++p)
-      umma_f16_ts(o_tmem + T::N64 * 64 + p * 16, a, desc_mn32(sB + T::part16_off(p), ks), idesc16, acc);
-  }
-}
-
-// all lanes of the load warp: element DH of every key row of a landed V tile := 1.0 (see FACfg::PAD_SUM)
-template <int DH>
-__device__ __forceinline__ void write_v_ones(uint8_t* sVstage, int lane) {
-  using X = FACfg<DH>;
-  constexpr int ch = DH / 8;  // the 16-byte chunk holding elements [DH, DH + 8): zero-filled by the TMA unit
-  for (int r = lane; r < X::BN; r += 32)
-    *reinterpret_cast<uint4*>(sVstage + sw128_chunk_off(r, ch)) = make_uint4(0x00003C00u, 0u, 0u, 0u);
-  fence_proxy_async();
-  __syncwarp();
-}
-
-template <int DH>
-__global__ void __launch_bounds__(kFThreads, FACfg<DH>::CTAS_PER_SM)
-spatial_attn_fwd_kernel(const __grid_constant__ CUtensorMap mq128, const __grid_constant__ CUtensorMap mk128,
-                        const __grid_constant__ CUtensorMap mv128, const __grid_constant__ CUtensorMap mq32,
-                        const __grid_constant__ CUtensorMap mk32, const __grid_constant__ CUtensorMap mv32,
-                        const FAParams prm) {
-  using X = FACfg<DH>;
-  using T = TileParts<DH>;
+  using TQ = typename X::TQ;
   using TK = typename X::TK;
-  constexpr int DHP = X::DHP, BN = X::BN, NS = X::NS;
+  constexpr int BN = kFBN, NS = X::NS;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = smem + X::OFF_Q;
-  uint8_t* sK = smem + X::OFF_K;   // NS stages
-  uint8_t* sV = smem + X::OFF_V;   // NS stages
+  uint8_t* sK = smem + X::OFF_K;  // NS stages
+  uint8_t* sV = smem + X::OFF_V;  // NS stages
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + X::OFF_BAR);
-  uint64_t* bar_q = bars + 0;        // Q landed                                         (tx)
-  uint64_t* s_full = bars + 1;       // [2] S_j in TMEM buffer j & 1                      (tcgen05.commit)
-  uint64_t* p_full = bars + 3;       // [2] P_j in TMEM buffer j & 1, S_j consumed        (4 warp arrivals)
-  uint64_t* pv_done = bars + 5;      // O += P_j V_j completed                            (tcgen05.commit)
-  uint64_t* kv_full = bars + 6;      // [NS] K_j and V_j landed in stage j % NS            (tx)
-  uint64_t* v_ready = bars + 10;     // [NS] ones column written into V_j (PAD_SUM)        (1 arrival)
-  uint64_t* stage_free = bars + 14;  // [NS] S_j and P V_j completed: stage j % NS may be refilled (tcgen05.commit)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
+  uint64_t* bar_q = bars;           // Q landed (tx)
+  uint64_t* full = bars + 1;        // [NS] K_j, V_j landed (tx)
+  uint64_t* empty = bars + 1 + NS;  // [NS] every consumer warp is done with stage j % NS
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int q0 = qt * kFM, N = prm.N;
-  const int T_tiles = (N + BN - 1) / BN;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * kFM;
+  const int T_tiles = (prm.Nk + BN - 1) / BN;
 
-  if (warp == kFMmaWarp) {
-    tmem_alloc<X::TCOLS>(tmem_slot);
+  if (tid == 0) {
+    mbar_init(bar_q, 1);
+    for (int i = 0; i < NS; ++i) mbar_init(full + i, 1), mbar_init(empty + i, kFWG * 4);
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == kFProducerWarp) {
     if (lane == 0) {
-      mbar_init(bar_q, 1), mbar_init(pv_done, 1);
-      for (int i = 0; i < 2; ++i) mbar_init(s_full + i, 1), mbar_init(p_full + i, 4);
-      for (int i = 0; i < NS; ++i) mbar_init(kv_full + i, 1), mbar_init(v_ready + i, 1), mbar_init(stage_free + i, 1);
-      fence_mbar_init();
       tma_prefetch_desc(&mq128), tma_prefetch_desc(&mk128), tma_prefetch_desc(&mv128);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == kFTmaWarp) {
-    // ================= load warp: lane 0 issues every TMA load; all lanes write the ones column =================
-    auto load_kv = [&](int j) {
-      const int st = j % NS;
-      mbar_arrive_expect_tx(kv_full + st, 2 * TK::BYTES);
-      tma_load_tile<DH, BN>(sK + st * TK::BYTES, &mk128, &mk32, kv_full + st, j * BN, h, b);
-      tma_load_tile<DH, BN>(sV + st * TK::BYTES, &mv128, &mv32, kv_full + st, j * BN, h, b);
-    };
-    if (lane == 0) {
-      mbar_arrive_expect_tx(bar_q, T::BYTES);
-      tma_load_tile<DH>(sQ, &mq128, &mq32, bar_q, q0, h, b);
-      for (int j = 0; j < NS && j < T_tiles; ++j) load_kv(j);
-    }
-    for (int j = 0; j < T_tiles; ++j) {
-      if constexpr (X::PAD_SUM) {
-        const int st = j % NS;
-        mbar_wait(kv_full + st, (j / NS) & 1);
-        write_v_ones<DH>(sV + st * TK::BYTES, lane);
-        if (lane == 0) mbar_arrive(v_ready + st);
-      }
-      if (j >= 1 && j - 1 + NS < T_tiles) {  // refill the stage of tile j - 1 once its MMAs have completed
-        mbar_wait(stage_free + (j - 1) % NS, ((j - 1) / NS) & 1);
-        if (lane == 0) load_kv(j - 1 + NS);
-      }
-      __syncwarp();
-    }
-  } else if (warp == kFMmaWarp) {
-    // ================= MMA warp: lane 0 issues every MMA =================
-    if (lane == 0) {
-      mbar_wait(bar_q, 0);
-      mbar_wait(kv_full, 0);
-      tc_fence_after();
-      issue_qk<DH>(tmem_base, smem_u32(sQ), smem_u32(sK));
-      umma_commit(s_full);
+      mbar_arrive_expect_tx(bar_q, TQ::BYTES);
+      tma_load_tile<DH, kFM>(sQ, &mq128, &mq32, bar_q, q0, h, b);
       for (int j = 0; j < T_tiles; ++j) {
-        const int st = j % NS, buf = j & 1;
-        if (j + 1 < T_tiles) {  // S_{j+1} into the other buffer while the softmax warps work on S_j
-          const int sn = (j + 1) % NS;
-          mbar_wait(kv_full + sn, ((j + 1) / NS) & 1);
-          tc_fence_after();
-          issue_qk<DH>(tmem_base + (buf ^ 1) * BN, smem_u32(sQ), smem_u32(sK + sn * TK::BYTES));
-          umma_commit(s_full + (buf ^ 1));
-        }
-        mbar_wait(p_full + buf, (j >> 1) & 1);  // every softmax thread has consumed S_j and written P_j
-        if constexpr (X::PAD_SUM) mbar_wait(v_ready + st, (j / NS) & 1);
-        tc_fence_after();
-        issue_pv<DH>(tmem_base + X::O_COL, tmem_base + buf * BN, smem_u32(sV + st * TK::BYTES), j > 0);
-        umma_commit(pv_done);
-        umma_commit(stage_free + st);
+        const int st = j % NS;
+        if (j >= NS) mbar_wait(empty + st, ((j / NS) - 1) & 1);
+        mbar_arrive_expect_tx(full + st, 2 * TK::BYTES);
+        tma_load_tile<DH, BN>(sK + st * X::KB, &mk128, &mk32, full + st, j * BN, h, b);
+        tma_load_tile<DH, BN>(sV + st * X::KB, &mv128, &mv32, full + st, j * BN, h, b);
       }
     }
-  } else {
-    // ================= softmax warps: thread = query row =================
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    const float c = prm.scale_log2e;
-    float m_used = -INFINITY, l_thr = 0.f;  // l_thr: thread-side row sum (unused when the V pad column carries it)
-    for (int j = 0; j < T_tiles; ++j) {
-      const uint32_t ph = j & 1;
-      const uint32_t sbuf = lane_addr + (j & 1) * BN;
-      mbar_wait(s_full + (j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t s[BN];
-#pragma unroll
-      for (int cc = 0; cc < BN / 32; ++cc) tmem_ld32(sbuf + cc * 32, s + cc * 32);
-      tmem_ld_wait();
+    return;
+  }
 
-      const int kvalid = N - j * BN;  // keys of this tile that exist (>= 1)
-      if (kvalid < BN) {
+  // ================= consumers: warpgroup wg owns query rows wg*64 .. wg*64 + 63 =================
+  const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+  const int row0 = q0 + wg * 64 + (warp & 3) * 16 + g;  // the thread's rows: row0, row0 + 8
+  const float c = prm.scale_log2e;
+  float o[X::ACC];
 #pragma unroll
-        for (int i = 0; i < BN; ++i)
-          if (i >= kvalid) s[i] = 0xff800000u;  // -inf
-      }
-      float mx0 = __uint_as_float(s[0]), mx1 = __uint_as_float(s[1]), mx2 = __uint_as_float(s[2]),
-            mx3 = __uint_as_float(s[3]);
+  for (int i = 0; i < X::ACC; ++i) o[i] = 0.f;
+  float m_[2] = {-INFINITY, -INFINITY}, l_[2] = {0.f, 0.f};  // running max (scaled, log2 units) and sum per row
+  mbar_wait(bar_q, 0);
+  const uint32_t aQ = smem_u32(sQ);
+
+  for (int j = 0; j < T_tiles; ++j) {
+    const int st = j % NS;
+    mbar_wait(full + st, (j / NS) & 1);
+    float s[BN / 2];
+    wg_fence();
+    gemm_kk<DH, kFM, BN>(s, aQ, wg * 64, smem_u32(sK + st * X::KB));
+    wg_commit();
+    wg_wait<0>();
+
+    const int kvalid = prm.Nk - j * BN;  // keys of this tile that exist (>= 1)
+    if (kvalid < BN) {
 #pragma unroll
-      for (int i = 4; i < BN; i += 4) {
-        mx0 = fmaxf(mx0, __uint_as_float(s[i])), mx1 = fmaxf(mx1, __uint_as_float(s[i + 1]));
-        mx2 = fmaxf(mx2, __uint_as_float(s[i + 2])), mx3 = fmaxf(mx3, __uint_as_float(s[i + 3]));
-      }
-      const float mxc = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * c;
-      if (j == 0) {
-        m_used = mxc;
-      } else {
-        const bool grow = mxc - m_used > kRescaleThreshold;
-        if (__any_sync(0xffffffffu, grow)) {
-          const float m_new = grow ? mxc : m_used;
-          const float alpha = ex2_approx(m_used - m_new);
-          m_used = m_new;
-          l_thr *= alpha;
-          mbar_wait(pv_done, ph ^ 1);  // O holds tiles 0..j-1 (P V_j cannot start before this warp's p_full arrival)
-          tc_fence_after();
+      for (int i = 0; i < BN / 2; ++i)
+        if ((i >> 2) * 8 + 2 * t + (i & 1) >= kvalid) s[i] = -INFINITY;
+    }
+    float negm[2];
 #pragma unroll
-          for (int cc = 0; cc < X::ACC_COLS / 16; ++cc) {
-            uint32_t r[16];
-            tmem_ld16(lane_addr + X::O_COL + cc * 16, r);
-            tmem_ld_wait();
+    for (int r = 0; r < 2; ++r) {
+      float mx = -INFINITY;
 #pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-            tmem_st16(lane_addr + X::O_COL + cc * 16, r);
-          }
-        }
-      }
-      // p = exp2(s*c - m_used), packed to fp16 pairs in place (s[0 .. BN/2) then hold the BN probabilities)
-      const float negm = -m_used;
-      float l0 = 0.f, l1 = 0.f;
+      for (int i = 0; i < BN / 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * r], s[4 * i + 2 * r + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_[r], mx * c);
+      const float alpha = ex2_approx(m_[r] - m_new);  // 0 on the first tile
+      m_[r] = m_new;
+      l_[r] *= alpha;
 #pragma unroll
-      for (int i = 0; i < BN; i += 2) {
+      for (int i = 0; i < X::ACC / 4; ++i) o[4 * i + 2 * r] *= alpha, o[4 * i + 2 * r + 1] *= alpha;
+      negm[r] = -m_new;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
         float p0, p1;
-        ex2_pair(i >> 1, __uint_as_float(s[i]), __uint_as_float(s[i + 1]), c, negm, p0, p1);
-        if constexpr (!X::PAD_SUM) l0 += p0, l1 += p1;
-        s[i >> 1] = pack_half2(p0, p1);
-      }
-      if constexpr (!X::PAD_SUM) l_thr += l0 + l1;
-      tmem_st32(sbuf, s);  // P over the consumed S (first BN / 2 columns of the buffer)
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full + (j & 1));
-    }
-    // ---- epilogue: O / l -> fp16 -> global; log-sum-exp for the backward ----
-    // S_{T-1} was issued BEFORE P V_{T-2}, so having consumed it only proves P V_{T-3} complete: a single parity wait for
-    // phase T-1 could be satisfied by the still-incomplete phase T-2 looking like "phase T-3 done". Wait for both in order.
-    if (T_tiles >= 2) mbar_wait(pv_done, (T_tiles - 2) & 1);
-    mbar_wait(pv_done, (T_tiles - 1) & 1);
-    tc_fence_after();
-    const int row = q0 + tid;
-    float l = l_thr;
-    if constexpr (X::PAD_SUM) {  // accumulator column DH = sum_j P_j * 1
-      uint32_t r[16];
-      tmem_ld16(lane_addr + X::O_COL + (DH / 16) * 16, r);
-      tmem_ld_wait();
-      l = __uint_as_float(r[DH % 16]);
-    }
-    const float inv = 1.f / l;
-    __half* orow = prm.o + (int64_t)b * prm.o_sb + (int64_t)row * prm.o_sr + h * DH;
-#pragma unroll
-    for (int cc = 0; cc < DHP / 16; ++cc) {
-      uint32_t r[16];
-      tmem_ld16(lane_addr + X::O_COL + cc * 16, r);
-      tmem_ld_wait();
-      if (row < N) {
-#pragma unroll
-        for (int half8 = 0; half8 < 2; ++half8) {
-          if (cc * 16 + half8 * 8 < DH) {
-            uint4 pk;
-            pk.x = pack_half2(__uint_as_float(r[half8 * 8 + 0]) * inv, __uint_as_float(r[half8 * 8 + 1]) * inv);
-            pk.y = pack_half2(__uint_as_float(r[half8 * 8 + 2]) * inv, __uint_as_float(r[half8 * 8 + 3]) * inv);
-            pk.z = pack_half2(__uint_as_float(r[half8 * 8 + 4]) * inv, __uint_as_float(r[half8 * 8 + 5]) * inv);
-            pk.w = pack_half2(__uint_as_float(r[half8 * 8 + 6]) * inv, __uint_as_float(r[half8 * 8 + 7]) * inv);
-            *reinterpret_cast<uint4*>(orow + cc * 16 + half8 * 8) = pk;
-          }
-        }
+        ex2_pair(i, s[4 * i + 2 * r], s[4 * i + 2 * r + 1], c, negm[r], p0, p1);
+        l_[r] += p0 + p1;
+        s[4 * i + 2 * r] = p0, s[4 * i + 2 * r + 1] = p1;
       }
     }
-    if (prm.lse != nullptr && row < N)
-      prm.lse[((int64_t)b * prm.H + h) * N + row] = (m_used + log2f(l)) * 0.6931471805599453f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kFMmaWarp) {
+    uint32_t pa[BN / 4];
+    acc_to_afrag<BN>(s, pa);
+    wg_fence();
+    gemm_rmn<DH, BN>(o, pa, smem_u32(sV + st * X::KB));
+    wg_commit();
+    wg_wait<0>();
     __syncwarp();
-    tmem_dealloc<X::TCOLS>(tmem_base);
+    if (lane == 0) mbar_arrive(empty + st);
+  }
+
+  // ---- epilogue: O / l -> fp16 -> global; log-sum-exp for the backward ----
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    const int row = row0 + 8 * r;
+    if (row < prm.Nq) {
+      __half* orow = prm.o + (int64_t)b * prm.o_sb + (int64_t)row * prm.o_sr + h * DH;
+#pragma unroll
+      for (int i = 0; i < X::ACC / 4; ++i) {
+        const int col = 8 * i + 2 * t;
+        if (col < DH) *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
+      }
+      if (prm.lse != nullptr && t == 0) prm.lse[((int64_t)b * prm.H + h) * prm.Nq + row] = (m_[r] + log2f(l)) * 0.6931471805599453f;
+    }
   }
 }
 
-struct AttnMaps {
-  CUtensorMap m128, m32;
-};
-
-// maps for one operand tensor (box height `rows`); the SW32 map is only encoded when the head dim has 16-wide parts
 template <int DH>
-static int make_maps(AttnMaps& m, const void* base, int H, int N, int B, int64_t sr, int64_t sb, int rows) {
-  using T = TileParts<DH>;
-  int rc = make_attn_tensor_map(&m.m128, base, DH, H, N, B, sr, sb, 64, rows, true);
-  if (rc) return rc;
-  if (T::N16 > 0) rc = make_attn_tensor_map(&m.m32, base, DH, H, N, B, sr, sb, 16, rows, false);
-  else m.m32 = m.m128;
-  return rc;
-}
-
-template <int DH>
-static int launch_spatial_fwd(const void* q, const void* k, const void* v, const FAParams& prm, int64_t q_sb, int64_t q_sr,
-                              int64_t k_sb, int64_t k_sr, int64_t v_sb, int64_t v_sr, cudaStream_t st) {
+static int launch_attn_fwd(const void* q, const void* k, const void* v, const FAParams& prm, int64_t q_sb, int64_t q_sr,
+                           int64_t k_sb, int64_t k_sr, int64_t v_sb, int64_t v_sr, cudaStream_t st) {
   using X = FACfg<DH>;
   AttnMaps mq, mk, mv;
-  if (make_maps<DH>(mq, q, prm.H, prm.N, prm.B, q_sr, q_sb, kFM) || make_maps<DH>(mk, k, prm.H, prm.N, prm.B, k_sr, k_sb, X::BN) ||
-      make_maps<DH>(mv, v, prm.H, prm.N, prm.B, v_sr, v_sb, X::BN)) {
+  if (make_attn_maps<DH>(mq, q, prm.H, prm.Nq, prm.B, q_sr, q_sb, kFM) ||
+      make_attn_maps<DH>(mk, k, prm.H, prm.Nk, prm.B, k_sr, k_sb, kFBN) ||
+      make_attn_maps<DH>(mv, v, prm.H, prm.Nk, prm.B, v_sr, v_sb, kFBN)) {
     return MC_E_CUDA;
   }
-  auto kern = spatial_attn_fwd_kernel<DH>;
+  const int q_tiles = (prm.Nq + kFM - 1) / kFM;
+  auto kern = attn_fwd_kernel<DH>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, X::SMEM);
-  dim3 grid((prm.N + kFM - 1) / kFM, prm.H, prm.B);
+  dim3 grid(q_tiles, prm.H, prm.B);
   kern<<<grid, kFThreads, X::SMEM, st>>>(mq.m128, mk.m128, mv.m128, mq.m32, mk.m32, mv.m32, prm);
   count_launch();
-  return check_launch("spatial_attn_fwd");
+  return check_launch("attn_fwd");
+}
+
+static int attn_fwd_dispatch(const char* what, int DH, const void* q, const void* k, const void* v, const FAParams& prm,
+                             int64_t q_sb, int64_t q_sr, int64_t k_sb, int64_t k_sr, int64_t v_sb, int64_t v_sr,
+                             cudaStream_t st) {
+#define MC_FA_CASE(D) \
+  case D: return launch_attn_fwd<D>(q, k, v, prm, q_sb, q_sr, k_sb, k_sr, v_sb, v_sr, st);
+  switch (DH) {
+    MC_FA_CASE(8) MC_FA_CASE(16) MC_FA_CASE(32) MC_FA_CASE(40) MC_FA_CASE(64) MC_FA_CASE(80) MC_FA_CASE(160)
+    default: break;
+  }
+#undef MC_FA_CASE
+  set_error("%s: unsupported head dim %d (8, 16, 32, 40, 64, 80, 160)", what, DH);
+  return MC_E_UNSUPPORTED;
 }
 
 }  // namespace mc
@@ -382,16 +233,37 @@ extern "C" int mc_spatial_attn_fwd(const void* q, const void* k, const void* v, 
   }
   FAParams prm{};
   prm.lse = lse, prm.o = (__half*)o, prm.o_sb = o_stride_b, prm.o_sr = o_stride_row;
-  prm.B = B, prm.N = N, prm.H = H;
+  prm.B = B, prm.Nq = N, prm.Nk = N, prm.H = H;
   prm.scale_log2e = scale * 1.44269504088896340736f;
-  cudaStream_t st = (cudaStream_t)stream;
-#define MC_SA_CASE(D) \
-  case D: return launch_spatial_fwd<D>(q, k, v, prm, q_stride_b, q_stride_row, k_stride_b, k_stride_row, v_stride_b, v_stride_row, st);
-  switch (DH) {
-    MC_SA_CASE(8) MC_SA_CASE(16) MC_SA_CASE(32) MC_SA_CASE(40) MC_SA_CASE(64) MC_SA_CASE(80) MC_SA_CASE(160)
-    default: break;
+  return attn_fwd_dispatch("spatial_attn_fwd", DH, q, k, v, prm, q_stride_b, q_stride_row, k_stride_b, k_stride_row,
+                           v_stride_b, v_stride_row, (cudaStream_t)stream);
+}
+
+extern "C" int mc_cross_attn_fwd(const void* q, const void* k, const void* v, void* o, int B, int Nq, int Nk, int H, int DH,
+                                 int64_t q_stride_b, int64_t q_stride_row, int64_t kv_stride_b, int64_t kv_stride_row,
+                                 int64_t o_stride_b, int64_t o_stride_row, float scale, void* stream) {
+  using namespace mc;
+  if (!q || !k || !v || !o || B <= 0 || Nq <= 0 || Nk <= 0 || H <= 0) {
+    set_error("cross_attn_fwd: null pointer or non-positive dims");
+    return MC_E_INVALID;
   }
-#undef MC_SA_CASE
-  set_error("spatial_attn_fwd: unsupported head dim %d (8, 16, 32, 40, 64, 80, 160)", DH);
-  return MC_E_UNSUPPORTED;
+  if (Nk > kMaxTextKeys) {
+    set_error("cross_attn_fwd: at most %d keys (text tokens), got %d", kMaxTextKeys, Nk);
+    return MC_E_UNSUPPORTED;
+  }
+  if (B > 65535 || H > 65535) {
+    set_error("cross_attn_fwd: at most 65535 batches / heads");
+    return MC_E_UNSUPPORTED;
+  }
+  if ((q_stride_row | kv_stride_row | o_stride_row | q_stride_b | kv_stride_b | o_stride_b) % 8 ||
+      ((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)o) % 16) {
+    set_error("cross_attn_fwd: pointers must be 16-byte aligned and strides multiples of 8 elements");
+    return MC_E_INVALID;
+  }
+  FAParams prm{};
+  prm.lse = nullptr, prm.o = (__half*)o, prm.o_sb = o_stride_b, prm.o_sr = o_stride_row;
+  prm.B = B, prm.Nq = Nq, prm.Nk = Nk, prm.H = H;
+  prm.scale_log2e = scale * 1.44269504088896340736f;
+  return attn_fwd_dispatch("cross_attn_fwd", DH, q, k, v, prm, q_stride_b, q_stride_row, kv_stride_b, kv_stride_row,
+                           kv_stride_b, kv_stride_row, (cudaStream_t)stream);
 }

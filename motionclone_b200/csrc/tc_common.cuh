@@ -1,97 +1,88 @@
-// tcgen05 / TMEM primitives shared by the attention kernels (sm_100a): shared-memory matrix descriptors for the
-// no-swizzle canonical layouts, the f16 instruction descriptor, single-thread MMA issue + commit, TMEM loads and fences.
-//   K-major  tile [R rows][K]: 16-byte chunk (row r, k-chunk c) at  c * (R*16) + r*16   (LBO = R*16, SBO = 128)
-//   MN-major tile [K rows][N]: 16-byte chunk (k-row j, n-chunk c) at c * (Kpad*16) + j*16 (SBO = Kpad*16, LBO = 128)
+// Warpgroup MMA (wgmma, sm_90a) primitives shared by the attention kernels: asynchronous m64nNk16 fp16 x fp16 -> fp32
+// with the B operand (and, for ss, the A operand) read from shared memory through a matrix descriptor, the A operand of
+// the rs form from registers. A warpgroup (4 consecutive warps, 128 threads) owns a 64-row accumulator: warp w of the
+// group holds rows 16w .. 16w + 15, and for every 8-column block i thread (g = lane / 4, t = lane % 4) holds
+//   d[4i + 0], d[4i + 1] = (row g,     columns 8i + 2t, 8i + 2t + 1)
+//   d[4i + 2], d[4i + 3] = (row g + 8, columns 8i + 2t, 8i + 2t + 1)
+// which is also the register layout of an A fragment (k16 step s: blocks 2s and 2s + 1), so a score tile turns into the
+// A operand of the next product without passing through shared memory.
 #pragma once
 #include "mc_common.cuh"
 
 namespace mc {
 
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // cute::UMMA::SmemDescriptor: start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1 layout_type[61,64)=0 (no swizzle)
+__device__ __forceinline__ void wgmma_ss_n32(float* d, uint64_t a, uint64_t b, int accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t a, uint64_t b, int accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_ss_n80(float* d, uint64_t a, uint64_t b, int accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(a), "l"(b), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_rs_n16(float* d, const uint32_t* a, uint64_t b, int accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_rs_n64(float* d, const uint32_t* a, uint64_t b, int accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accum));
+}
+
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b, int accum) {
+  static_assert(N == 32 || N == 64 || N == 80, "wgmma_ss: N in {32, 64, 80}");
+  if constexpr (N == 32) wgmma_ss_n32(d, a, b, accum);
+  else if constexpr (N == 64) wgmma_ss_n64(d, a, b, accum);
+  else wgmma_ss_n80(d, a, b, accum);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t b, int accum) {
+  static_assert(N == 16 || N == 64, "wgmma_rs: N in {16, 64}");
+  if constexpr (N == 16) wgmma_rs_n16(d, a, b, accum);
+  else wgmma_rs_n64(d, a, b, accum);
+}
+
+// register writes (accumulators, A fragments) -> visible to the next wgmma; group bookkeeping
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+
+// shared-memory matrix descriptor: start[0,14) lbo[16,30) sbo[32,46) (all >> 4), base offset[49,52) = 0 (every swizzle
+// atom used here is aligned to its own size), layout[62,64): 1 = 128-byte swizzle, 3 = 32-byte swizzle
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
+  d |= (uint64_t)layout << 62;
   return d;
 }
 
-__device__ __forceinline__ uint32_t umma_instr_desc_f16(int M, int N, bool b_mn_major) {
-  // cute::UMMA::InstrDescriptor: c_format[4,6)=1 (F32), a/b_format = 0 (F16), a_major[15], b_major[16], n>>3 [17,23), m>>4 [24,29)
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (b_mn_major ? 1u : 0u) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
-}
-
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Stage NROWS rows (first global row `row0`, rows >= nvalid are zero-filled) of head-columns [0, DH) of a row-major
-// global tensor into the K-major / MN-major no-swizzle chunk layout: 16-byte chunk (row r, chunk c) at (c*R + r)*16.
-// Consecutive threads read consecutive 16-byte chunks of a row (coalesced); chunks >= DH/8 (the K padding) are zeros.
-// Loads are issued in batches of 8 per thread before the first shared-memory store (8 x 16 B in flight per thread).
-template <int DH, int KCQ, int R, int NROWS, int NTHR>
-__device__ __forceinline__ void stage_chunks(uint8_t* sdst, const __half* gsrc, int64_t row_stride, int row0, int nvalid,
-                                             int tid) {
-  constexpr int KC = DH / 8;  // real chunks per row
-  constexpr int TOTAL = NROWS * KC;
-  constexpr int ITERS = (TOTAL + NTHR - 1) / NTHR;
-  constexpr int UN = 8;
+// fp32 accumulator (rows g, g + 8 of the thread) -> A fragments of KR / 16 k16 steps, fp16 pairs
+template <int KR>
+__device__ __forceinline__ void acc_to_afrag(const float* s, uint32_t* a) {
 #pragma unroll
-  for (int it0 = 0; it0 < ITERS; it0 += UN) {
-    uint4 vals[UN];
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      const int i = tid + (it0 + u) * NTHR;
-      vals[u] = make_uint4(0u, 0u, 0u, 0u);
-      if (it0 + u < ITERS && i < TOTAL) {
-        const int r = i / KC, c = i % KC;
-        if (row0 + r < nvalid) vals[u] = *reinterpret_cast<const uint4*>(gsrc + (int64_t)(row0 + r) * row_stride + c * 8);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      const int i = tid + (it0 + u) * NTHR;
-      if (it0 + u < ITERS && i < TOTAL) {
-        const int r = i / KC, c = i % KC;
-        *reinterpret_cast<uint4*>(sdst + (c * R + r) * 16) = vals[u];
-      }
-    }
-  }
-  if (KCQ > KC) {  // zero the padding chunk(s)
-    for (int i = tid; i < NROWS * (KCQ - KC); i += NTHR) {
-      const int r = i % NROWS, c = KC + i / NROWS;
-      *reinterpret_cast<uint4*>(sdst + (c * R + r) * 16) = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
+  for (int i = 0; i < KR / 2; i += 2) a[i / 2] = pack_half2(s[i], s[i + 1]);
 }
 
 }  // namespace mc

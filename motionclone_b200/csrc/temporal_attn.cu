@@ -1,16 +1,16 @@
-// Fused temporal self-attention over the frame axis (forward + backward) for sm_100a.
+// Fused temporal self-attention over the frame axis (forward + backward) for sm_90a.
 //
 // Replaces VersatileAttention's core (reference models/motion_module.py:309-332 -> models/attention.py:461-490), the
 // second softmax pass of get_temp_attn_prob (utils/motionclone_functions.py:260-283 -> models/attention.py:564-611),
 // torch.topk(k=1) (utils/motionclone_functions.py:79) and torch.gather (…:92) — one pass over Q, K, V.
 //
 // Shape of the problem: per (batch, position, head) a 16x16 (L x L, L in {8,16,32}) attention with DH in [8,160]:
-// arithmetic intensity L/2 flop/byte => HBM-bound (DESIGN.md §3). One CTA stages a tile of
+// arithmetic intensity L/2 flop/byte => HBM-bound (DESIGN.md §4, T1/T2). One CTA stages a tile of
 // (all L frames) x (P positions) x (HG heads) of Q, K, V in shared memory with 1-D bulk copies (TMA engine, UBLKCP)
 // signalled on mbarriers; each warp owns (position, head) items: QK^T, the fp16-rounded softmax and PV run on
 // m16n8k16 tensor-core fragments straight out of ldmatrix, O is written back over Q's tile and leaves with bulk
-// stores. A tcgen05 tile (M >= 64) would have to pad 16-row problems 4-8x and round-trip TMEM for an op that has
-// 8 flop/byte to spend; see DESIGN.md §3 for the arithmetic behind this choice.
+// stores. A wgmma tile (M >= 64) would have to pad 16-row problems 4-8x for an op that has
+// 8 flop/byte to spend; see DESIGN.md §4 (T1/T2) for the arithmetic behind this choice.
 //
 // The frame pitch in shared memory is padded to 16 (mod 128) bytes so the 8 row addresses of every ldmatrix phase
 // fall in 8 different 16 B bank groups (rows of one (position, head) item are `pitch` apart).
@@ -695,7 +695,7 @@ static int pad16(int row_bytes) { return row_bytes + ((16 - (row_bytes % 128)) +
 static bool choose_geom(int D, int L, int H, int DH, int ntensors, bool need_even_p, bool fusable, TileGeom* g,
                         int n_batch = 0) {
   // Tile size: ~32 KB per Q/K/V set keeps 6-7 CTAs resident per SM (227 KB), which is what de-synchronises their
-  // load / math / store phases (measured on B200: 61 KB tiles reach 54 % of the HBM roof at C=320, 30 KB tiles 62-75 %).
+  // load / math / store phases.
   // Tiles that would hold fewer than 4 (position, head) items get twice the budget instead of idle warps.
   const int base = 32 * 1024 * ntensors / 3;
   auto tbytes = [&](int P, int hg) { return (int64_t)ntensors * L * P * hg * DH * 2; };
@@ -716,7 +716,7 @@ static bool choose_geom(int D, int L, int H, int DH, int ntensors, bool need_eve
   // warps of a CTA then idle, which costs nothing here) until the launch has at least two waves of resident CTAs.
   if (n_batch > 0) {
     auto ctas = [&](int hg) { return (int64_t)n_batch * (D / P) * (H / hg); };
-    auto resident = [&](int hg) { return (int64_t)148 * (227 * 1024 / (tbytes(P, hg) + 2048)); };
+    auto resident = [&](int hg) { return (int64_t)132 * (227 * 1024 / (tbytes(P, hg) + 2048)); };
     while (HG > 2 && HG % 2 == 0 && ctas(HG) < 2 * resident(HG)) HG /= 2;
   }
   g->P = P;

@@ -1,14 +1,14 @@
-// TMA tensor maps (cp.async.bulk.tensor, SASS UTMALDG) + swizzled UMMA shared-memory descriptors, sm_100a.
+// TMA tensor maps (cp.async.bulk.tensor) + swizzled wgmma shared-memory descriptors, sm_90a.
 //
-// An attention operand tile is [128 rows][DH] fp16 (rows = tokens of one frame / head, DH contiguous in global memory).
+// An attention operand tile is [ROWS][DH] fp16 (rows = tokens of one frame / head, DH contiguous in global memory).
 // In shared memory it is a sequence of PARTS along DH, each landed by ONE tensor-map load:
-//   SW128 part: [128 rows][64 elements = 128 B], CU_TENSOR_MAP_SWIZZLE_128B   (16 KB; 1024-byte aligned)
-//   SW32  part: [128 rows][16 elements =  32 B], CU_TENSOR_MAP_SWIZZLE_32B    ( 4 KB)
-// DH = 40 -> one SW128 part whose columns 40..63 are zero-filled by the TMA unit (the map's innermost extent is DH, the
+//   SW128 part: [ROWS][64 elements = 128 B], CU_TENSOR_MAP_SWIZZLE_128B   (1024-byte aligned)
+//   SW32  part: [ROWS][16 elements =  32 B], CU_TENSOR_MAP_SWIZZLE_32B
+// DH < 64 -> one SW128 part whose columns DH..63 are zero-filled by the TMA unit (the map's innermost extent is DH, the
 // box is 64 wide: out-of-bounds elements read as 0); DH = 80 -> SW128 + SW32; DH = 160 -> 2 x SW128 + 2 x SW32.
 // The same bytes serve as
 //   K-major operand  (rows = M or N, DH = K):  canonical  Swizzle<3,4,3> o ((8,n),2):((8,SBO),1)   [units of 16 B]
-//   MN-major operand (DH = M or N, rows = K):  canonical  Swizzle<3,4,3> o ((8,n),(8,k)):((1,LBO),(8,SBO))
+//   MN-major operand (DH = N, rows = K):       canonical  Swizzle<3,4,3> o ((8,n),(8,k)):((1,LBO),(8,SBO))
 // so V needs no transpose for P V, and K / Q / dO tiles are shared between the GEMMs of the backward pass.
 #pragma once
 #include <cuda.h>
@@ -65,6 +65,22 @@ inline int make_attn_tensor_map(CUtensorMap* map, const void* base, int DH, int 
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
+// Text cross-attention takes the whole key axis (77 tokens) as one tile in the backward: at most this many keys.
+constexpr int kMaxTextKeys = 80;
+
+struct AttnMaps {
+  CUtensorMap m128, m32;
+};
+// maps for one operand tensor (box height `rows`); the SW32 map is only encoded when the head dim has 16-wide parts
+template <int DH>
+int make_attn_maps(AttnMaps& m, const void* base, int H, int N, int B, int64_t sr, int64_t sb, int rows) {
+  int rc = make_attn_tensor_map(&m.m128, base, DH, H, N, B, sr, sb, 64, rows, true);
+  if (rc) return rc;
+  if (DH >= 64 && DH % 64 != 0) rc = make_attn_tensor_map(&m.m32, base, DH, H, N, B, sr, sb, 16, rows, false);
+  else m.m32 = m.m128;
+  return rc;
+}
+
 // ---- device: tensor-map load into shared memory, completion on an mbarrier ----
 __device__ __forceinline__ void tma_load_4d(void* sdst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
@@ -77,7 +93,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// ---- operand-tile geometry ----
+// ---- operand-tile geometry (the row count of a tile is a multiple of 8: whole swizzle atoms) ----
 template <int DH, int ROWS = 128>
 struct TileParts {
   static_assert(DH % 8 == 0, "head dim must be a multiple of 8 (16-byte rows)");
@@ -108,107 +124,60 @@ __device__ __forceinline__ void tma_load_tile(uint8_t* sdst, const CUtensorMap* 
   for (int p = 0; p < T::N16; ++p) tma_load_4d(sdst + T::part16_off(p), map32, bar, T::N64 * 64 + p * 16, h, r0, b);
 }
 
-// ---- swizzled shared-memory descriptors (cute::UMMA::SmemDescriptor, version 1) ----
-//   layout_type [61,64): 2 = SWIZZLE_128B, 6 = SWIZZLE_32B
-__device__ __forceinline__ uint64_t umma_desc_sw(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
-}
+// ---- swizzled wgmma descriptors ----
 // K-major SW128 part, k16 step ks (0..3): rows 128 B apart, 8-row groups 1024 B apart, 32 B per k step
-__device__ __forceinline__ uint64_t desc_k128(uint32_t part_addr, int ks) {
-  return umma_desc_sw(part_addr + ks * 32, 16, 1024, 2);
-}
+__device__ __forceinline__ uint64_t desc_k128(uint32_t part_addr, int ks) { return gmma_desc(part_addr + ks * 32, 16, 1024, 1); }
 // K-major SW32 part (one k16 step): rows 32 B apart, 8-row groups 256 B apart
-__device__ __forceinline__ uint64_t desc_k32(uint32_t part_addr) { return umma_desc_sw(part_addr, 16, 256, 6); }
-// MN-major SW128 part, k16 step ks over the ROWS (16 rows = 2048 B): 8-row groups 1024 B apart; 64-element MN atoms
-// `lbo_bytes` apart (only read when the MMA's M / N extent exceeds 64)
-__device__ __forceinline__ uint64_t desc_mn128(uint32_t part_addr, int ks, uint32_t lbo_bytes = 16384) {
-  return umma_desc_sw(part_addr + ks * 2048, lbo_bytes, 1024, 2);
-}
+__device__ __forceinline__ uint64_t desc_k32(uint32_t part_addr) { return gmma_desc(part_addr, 16, 256, 3); }
+// MN-major SW128 part (64 elements wide), k16 step ks over the ROWS (16 rows = 2048 B): 8-row groups 1024 B apart
+__device__ __forceinline__ uint64_t desc_mn128(uint32_t part_addr, int ks) { return gmma_desc(part_addr + ks * 2048, 16384, 1024, 1); }
 // MN-major SW32 part (16 elements wide), k16 step ks over the rows (16 rows = 512 B): 8-row groups 256 B apart
-__device__ __forceinline__ uint64_t desc_mn32(uint32_t part_addr, int ks) {
-  return umma_desc_sw(part_addr + ks * 512, 4096, 256, 6);
-}
+__device__ __forceinline__ uint64_t desc_mn32(uint32_t part_addr, int ks) { return gmma_desc(part_addr + ks * 512, 4096, 256, 3); }
 
-// instruction descriptor with both majors selectable (bit 15: A is MN-major, bit 16: B is MN-major)
-__device__ __forceinline__ uint32_t umma_idesc_f16(int M, int N, bool a_mn, bool b_mn) {
-  uint32_t d = 0;
-  d |= 1u << 4;  // fp32 accumulate
-  d |= (a_mn ? 1u : 0u) << 15;
-  d |= (b_mn ? 1u : 0u) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
-}
+__host__ __device__ constexpr int align1k(int bytes) { return (bytes + 1023) / 1024 * 1024; }
 
-// byte offset of (row r, 16-byte chunk c of 8) inside a K-major SW128 part written by threads (P, dS tiles)
-__device__ __forceinline__ uint32_t sw128_chunk_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
-
-// ---- TMEM 32-column load / 16-column store (32x32b: thread = lane = row) ----
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-// one row (DHP fp16, DHP % 16 == 0) of a K-major SW128 tile part in shared memory -> DHP / 2 packed TMEM columns of the
-// calling thread's lane: how a resident [128][DH <= 48] operand tile becomes a tensor-memory A operand
-template <int DHP>
-__device__ __forceinline__ void smem_row_to_tmem(const uint8_t* part, int r, uint32_t taddr) {
-  static_assert(DHP % 16 == 0 && DHP <= 64, "one SW128 part");
-  uint32_t v[DHP / 2];
+// D[64 x BN] (+)= A B^T with A = rows arow0 .. arow0 + 63 of an [AROWS][DH] tile and B = a [BN][DH] tile, both K-major
+// (the head dim is contracted). Issues the wgmma chain; the caller fences, commits and waits.
+template <int DH, int AROWS, int BN>
+__device__ __forceinline__ void gemm_kk(float* d, uint32_t sA, int arow0, uint32_t sB) {
+  using TA = TileParts<DH, AROWS>;
+  using TB = TileParts<DH, BN>;
+  int acc = 0;
 #pragma unroll
-  for (int c = 0; c < DHP / 8; ++c) {
-    const uint4 x = *reinterpret_cast<const uint4*>(part + sw128_chunk_off(r, c));
-    v[4 * c] = x.x, v[4 * c + 1] = x.y, v[4 * c + 2] = x.z, v[4 * c + 3] = x.w;
+  for (int p = 0; p < TA::N64; ++p)
+#pragma unroll
+    for (int ks = 0; ks < TA::KS64; ++ks) {
+      wgmma_ss<BN>(d, desc_k128(sA + TA::part64_off(p) + arow0 * 128, ks), desc_k128(sB + TB::part64_off(p), ks), acc);
+      acc = 1;
+    }
+#pragma unroll
+  for (int p = 0; p < TA::N16; ++p) {
+    wgmma_ss<BN>(d, desc_k32(sA + TA::part16_off(p) + arow0 * 32), desc_k32(sB + TB::part16_off(p)), acc);
+    acc = 1;
   }
+}
+
+// D[64 x ACC_W] (+)= A B with A = fp16 fragments in registers (KR / 16 k16 steps of 4 registers) and B = a [KR][DH] tile
+// read MN-major (its rows are contracted). ACC_W = 64 per SW128 part (columns past DH come out as 0) + 16 per SW32 part;
+// the accumulator's 8-column block i is output columns 8i .. 8i + 7 across the parts.
+template <int DH>
+struct AccW {
+  using T = TileParts<DH, 64>;
+  static constexpr int W = T::N64 * 64 + T::N16 * 16;
+  static constexpr int REGS = W / 2;
+};
+template <int DH, int KR>
+__device__ __forceinline__ void gemm_rmn(float* d, const uint32_t* a, uint32_t sB) {
+  using TB = TileParts<DH, KR>;
 #pragma unroll
-  for (int c = 0; c < DHP / 16; ++c) tmem_st8(taddr + c * 8, v + c * 8);
+  for (int ks = 0; ks < KR / 16; ++ks) {
+#pragma unroll
+    for (int p = 0; p < TB::N64; ++p) wgmma_rs<64>(d + p * 32, a + 4 * ks, desc_mn128(sB + TB::part64_off(p), ks), 1);
+#pragma unroll
+    for (int p = 0; p < TB::N16; ++p)
+      wgmma_rs<16>(d + TB::N64 * 32 + p * 8, a + 4 * ks, desc_mn32(sB + TB::part16_off(p), ks), 1);
+  }
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-      "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-      "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// D (+)= A B with A in TENSOR MEMORY (fp16 pairs: lane = row m, 32-bit column j = elements k = 2j, 2j + 1; 8 columns per
-// k16 step) and B through a shared-memory descriptor: P / dS tiles never round-trip through shared memory.
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -216,41 +185,25 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// exp2 of a PAIR on the FMA pipe (FADD2 / FFMA2, two fp32 lanes per instruction) instead of the 16-lane/clk MUFU: the
-// attention kernels are bound by MUFU.EX2 issue, the FMA pipe idles, so a fixed fraction of the pairs goes this way.
-// x = n + f with n = round(x) by the 1.5 * 2^23 trick (the integer lands in the low mantissa bits), 2^f on [-0.5, 0.5] by
-// the degree-4 minimax polynomial (max relative error 2.7e-6, the probabilities are rounded to fp16, half-ulp 4.9e-4,
-// right after; degree 3, 7.5e-5, moved the 32-frame extraction's top-1 agreement with the oracle measurably), 2^n by adding n << 23 to the exponent field. Inputs are clamped at -126 (result 2^-126: 0 in fp16).
-__device__ __forceinline__ void ex2_poly_pair(float s0, float s1, float c, float negm, float& p0, float& p1) {
-  uint64_t sp, cc, mm, x, t, f, p;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(sp) : "f"(s0), "f"(s1));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(cc) : "f"(c));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(mm) : "f"(negm));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(x) : "l"(sp), "l"(cc), "l"(mm));
-  float x0, x1;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(x0), "=f"(x1) : "l"(x));
-  x0 = fmaxf(x0, -126.f), x1 = fmaxf(x1, -126.f);
-  asm("mov.b64 %0, {%1, %2};" : "=l"(x) : "f"(x0), "f"(x1));
-  uint64_t magic, nmagic, k4, k3, k2, k1, k0;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(magic) : "f"(12582912.f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(nmagic) : "f"(-12582912.f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(k4) : "f"(0.009570101276040077f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(k3) : "f"(0.05591786280274391f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(k2) : "f"(0.240247443318367f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(k1) : "f"(0.6931217908859253f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(k0) : "f"(0.9999992847442627f));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(t) : "l"(x), "l"(magic));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(f) : "l"(t), "l"(nmagic));   // n = round(x)
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(f) : "l"(x), "l"(f));        // f = x - n
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p) : "l"(k4), "l"(f), "l"(k3));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p) : "l"(p), "l"(f), "l"(k2));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p) : "l"(p), "l"(f), "l"(k1));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p) : "l"(p), "l"(f), "l"(k0));
-  float q0, q1, t0, t1;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(q0), "=f"(q1) : "l"(p));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(t0), "=f"(t1) : "l"(t));
-  p0 = __uint_as_float(__float_as_uint(q0) + (__float_as_uint(t0) << 23));
-  p1 = __uint_as_float(__float_as_uint(q1) + (__float_as_uint(t1) << 23));
+// exp2 on the FMA pipe instead of the MUFU unit, for a fixed fraction of the softmax exponentials (the two units then
+// share the work). x = n + f with n = round(x) by the 1.5 * 2^23 trick (the integer lands in the low mantissa bits),
+// 2^f on [-0.5, 0.5] by the degree-4 minimax polynomial (max relative error 2.7e-6; the probabilities are rounded to fp16,
+// half-ulp 4.9e-4, right after), 2^n by adding n << 23 to the exponent field. Inputs are clamped at -126 (result 2^-126:
+// 0 in fp16).
+__device__ __forceinline__ float ex2_poly(float s, float c, float negm) {
+  constexpr float k4 = 0.009570101276040077f;
+  constexpr float k3 = 0.05591786280274391f;
+  constexpr float k2 = 0.240247443318367f;
+  constexpr float k1 = 0.6931217908859253f;
+  constexpr float k0 = 0.9999992847442627f;
+  const float x = fmaxf(fmaf(s, c, negm), -126.f);
+  const float t = __fadd_rn(x, 12582912.f);
+  const float f = __fsub_rn(x, __fadd_rn(t, -12582912.f));  // f = x - round(x)
+  float p = fmaf(k4, f, k3);
+  p = fmaf(p, f, k2);
+  p = fmaf(p, f, k1);
+  p = fmaf(p, f, k0);
+  return __uint_as_float(__float_as_uint(p) + (__float_as_uint(t) << 23));
 }
 // Every MC_EX2_POLY_PERIOD-th pair of an unrolled softmax loop takes the polynomial (0: none).
 #ifndef MC_EX2_POLY_PERIOD
@@ -258,22 +211,12 @@ __device__ __forceinline__ void ex2_poly_pair(float s0, float s1, float c, float
 #endif
 __device__ __forceinline__ void ex2_pair(int pair_index, float s0, float s1, float c, float negm, float& p0, float& p1) {
   if (MC_EX2_POLY_PERIOD > 0 && pair_index % (MC_EX2_POLY_PERIOD > 0 ? MC_EX2_POLY_PERIOD : 1) == (MC_EX2_POLY_PERIOD - 1)) {
-    ex2_poly_pair(s0, s1, c, negm, p0, p1);
+    p0 = ex2_poly(s0, c, negm);
+    p1 = ex2_poly(s1, c, negm);
   } else {
     p0 = ex2_approx(fmaf(s0, c, negm));
     p1 = ex2_approx(fmaf(s1, c, negm));
   }
-}
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t base) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "n"(COLS) : "memory");
 }
 
 }  // namespace mc

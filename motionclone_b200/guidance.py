@@ -1,4 +1,4 @@
-"""The nine MotionClone functions, B200-native, with the reference's names and signatures.
+"""The nine MotionClone functions, H100-native (sm_90a), with the reference's names and signatures.
 
 The reference keeps its algorithm in nine free functions (motionclone/utils/motionclone_functions.py) that the entry
 scripts bind onto the pipeline / scheduler / unet instances with `fn.__get__(obj)` (t2v_video_sample.py:57-65). The
@@ -8,7 +8,7 @@ same nine names live here and bind the same way (`bind_motionclone` does the t2v
     sample_video                   :102   single_step_video            :173   get_temp_attn_prob  :260
     schedule_customized_step       :285   schedule_set_timesteps       :413   unet_customized_forward :478
 
-What changes underneath (DESIGN.md §4):
+What changes underneath (DESIGN.md §4 T1/T2 and §5):
   * one fused temporal-attention kernel emits the attention output AND the top-1 pair (extraction) or the
     probabilities gathered at the reference indices (guided steps): no second softmax pass, no [N,8,L,L] tensor,
     no topk / gather launches; the loss and its closed-form gradient are two small launches;

@@ -516,7 +516,7 @@ def _check_xattn(q: Tensor, k: Tensor, v: Tensor) -> None:
 
 
 def cross_attention_forward(q: Tensor, k: Tensor, v: Tensor, heads: int, scale: float) -> Tensor:
-    """tcgen05 text cross-attention (csrc/cross_attn_fwd_tc.cu, csrc/cross_attn_bwd_tc.cu): q [B, Nq, C], k / v [B, Nk <= 80, C] -> [B, Nq, C]."""
+    """wgmma text cross-attention (csrc/spatial_attn_tc.cu, csrc/spatial_attn_bwd_tc.cu): q [B, Nq, C], k / v [B, Nk <= 80, C] -> [B, Nq, C]."""
     _check_xattn(q, k, v)
     B, Nq, C = q.shape
     o = torch.empty((B, Nq, C), dtype=q.dtype, device=q.device)
@@ -551,7 +551,7 @@ def cross_attention_backward(q: Tensor, k: Tensor, v: Tensor, d_o: Tensor, heads
 
 
 class CrossAttentionTC(torch.autograd.Function):
-    """o = softmax(scale q k^T) v on the tcgen05 kernels, differentiable w.r.t. q only (see mc_cross_attn_bwd_dq)."""
+    """o = softmax(scale q k^T) v on the wgmma kernels, differentiable w.r.t. q only (see mc_cross_attn_bwd_dq)."""
 
     @staticmethod
     def forward(ctx, q, k, v, heads: int, scale: float):
@@ -569,7 +569,7 @@ class CrossAttentionTC(torch.autograd.Function):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# spatial self-attention (tcgen05 + tensor-map TMA flash kernel, csrc/spatial_attn_tc.cu)
+# spatial self-attention (wgmma + tensor-map TMA flash kernel, csrc/spatial_attn_tc.cu)
 # ----------------------------------------------------------------------------------------------------------------
 SPATIAL_ATTN_HEAD_DIMS = (8, 16, 32, 40, 64, 80, 160)
 
@@ -631,7 +631,7 @@ def spatial_attention_backward(q: Tensor, k: Tensor, v: Tensor, o: Tensor, lse: 
 
 
 class SpatialAttentionTC(torch.autograd.Function):
-    """O = softmax(scale Q K^T) V per (frame, head) on the tcgen05 kernels, forward and backward.
+    """O = softmax(scale Q K^T) V per (frame, head) on the wgmma kernels, forward and backward.
     q, k, v: [B, N, C] views; when they are the column blocks of one fused [B, N, 3C] tensor autograd accumulates the
     three returned gradient views into that tensor's gradient."""
 

@@ -4,17 +4,17 @@ Interface and state-dict keys follow the reference's motionclone/models/attentio
 BasicTransformerBlock (:145), CrossAttention (:302), plus diffusers-0.16's FeedForward/GEGLU that the reference
 imports (:14; keys ff.net.0.proj.*, ff.net.2.*).
 
-Design differences (B200-first):
+Design differences:
 * tokens `[(b f), h*w, C]` are a zero-copy view of the channels_last activation; proj_in/proj_out (1x1 convs in the
   checkpoint, `use_linear_projection=False`) run as GEMMs on that view;
 * self-attention projects q,k,v with one GEMM; cross-attention projects the text K/V ONCE per prompt, not once per
   frame (the reference repeats the text f times, attention.py:100, and re-projects it for every frame);
-* text cross-attention (`attn2`) runs on this package's tcgen05 / TMEM kernels (csrc/cross_attn_fwd_tc.cu, csrc/cross_attn_bwd_tc.cu), forward and
+* text cross-attention (`attn2`) runs on this package's wgmma attention kernels (csrc/spatial_attn_tc.cu, csrc/spatial_attn_bwd_tc.cu), forward and
   the gradient w.r.t. the queries (the text K / V carry no gradient on the MotionClone path);
 * spatial SELF-attention at the reference's xformers seam (`_memory_efficient_attention_xformers`, :535-542) runs on this
-  package's tcgen05 + tensor-map TMA flash kernels (csrc/spatial_attn_tc.cu), forward and backward (dQ, dK, dV);
+  package's wgmma + tensor-map TMA flash kernels (csrc/spatial_attn_tc.cu), forward and backward (dQ, dK, dV);
 * there is no ATen / library fallback on this path: CPU tensors, fp32 activations, trainable norm weights or shapes
-  outside the compiled instantiations raise (DESIGN.md §4).
+  outside the compiled instantiations raise (DESIGN.md §5).
 """
 from __future__ import annotations
 
@@ -267,7 +267,7 @@ class CrossAttention(nn.Module):
         inner = self.to_q.out_features
         dh = inner // h
         if encoder_hidden_states is None:
-            # spatial self-attention: one fused QKV GEMM, then the tcgen05 + TMA flash kernels on its column blocks
+            # spatial self-attention: one fused QKV GEMM, then the wgmma + TMA flash kernels on its column blocks
             qkv = F.linear(hidden_states, self.fused_qkv_weight())  # [(b f), N, 3C]
             if self.processor is not None:
                 self.processor.record_qkv(self, hidden_states, qkv[..., :inner], qkv[..., inner:2 * inner],
@@ -289,7 +289,7 @@ class CrossAttention(nn.Module):
             if ctx.shape[1] > 80 or dh not in _XATTN_TC_HEAD_DIMS or (torch.is_grad_enabled() and kv.requires_grad):
                 raise NotImplementedError("text cross-attention kernel: <= 80 context tokens, head dim in "
                                           f"{_XATTN_TC_HEAD_DIMS}, frozen K / V projections of a constant prompt")
-            # tcgen05 / TMEM kernels (csrc/cross_attn_{fwd,bwd}_tc.cu); dQ only: the text K / V carry no gradient here
+            # wgmma kernels (csrc/spatial_attn_tc.cu, csrc/spatial_attn_bwd_tc.cu); dQ only: the text K / V carry no gradient here
             if torch.is_grad_enabled() and q.requires_grad:
                 o = ops.CrossAttentionTC.apply(q, k, v, h, self.scale)
             else:

@@ -1,4 +1,4 @@
-"""Motion module (AnimateDiff temporal transformer) on the B200 kernels.
+"""Motion module (AnimateDiff temporal transformer) on this package's CUDA kernels.
 
 Mirrors the reference interface of motionclone/models/motion_module.py — VanillaTemporalModule (:51),
 TemporalTransformer3DModel (:88), TemporalTransformerBlock (:164), PositionalEncoding (:228), VersatileAttention (:250)

@@ -5,7 +5,7 @@ unet_blocks.py, resnet.py) so SD1.5 + AnimateDiff checkpoints map one to one. Th
 (utils/motionclone_functions.py:478-662): autograd only up to the last guidance block, `only_motion_feature` early
 exit, ControlNet residual inputs.
 
-B200-first layout: between blocks the activation is ONE 4-D tensor `[(b f), C, h, w]` in torch.channels_last, i.e.
+Layout: between blocks the activation is ONE 4-D tensor `[(b f), C, h, w]` in torch.channels_last, i.e.
 physically `[(b f), h, w, C]`. Consequences:
   * the reference's "b c f h w <-> (b f) c h w" rearranges around every conv / norm (resnet.py:14-16, 24-26) vanish;
   * cuDNN runs NHWC tensor-core convolutions with no layout transposes;

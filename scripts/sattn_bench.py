@@ -1,4 +1,4 @@
-"""Microbenchmark: this package's tcgen05 + TMA spatial self-attention against the library SDPA kernels on the UNet's
+"""Microbenchmark: this package's wgmma + TMA spatial self-attention against the library SDPA kernels on the UNet's
 shapes (forward; forward + backward when the backward kernels exist). Profiling aid, not a bench value."""
 import json
 import sys
@@ -8,7 +8,7 @@ import torch
 import torch.nn.functional as F
 from motionclone_b200 import _lib, ops
 
-# `--lib PATH`: time a side-by-side build of the same sources (scripts/build_variant.sh) instead of the in-tree library
+# `--lib PATH`: time a side-by-side build of the same sources instead of the in-tree library
 if "--lib" in sys.argv:
     i = sys.argv.index("--lib")
     _lib.LIB_PATH = os.path.abspath(sys.argv[i + 1])
@@ -32,7 +32,7 @@ def bench(fn, n=20):
 
 shapes = [("self64", 16, 8, 4096, 40), ("self32", 16, 8, 1024, 80), ("self16", 16, 8, 256, 160), ("self8", 16, 8, 64, 160),
           ("self64_b2", 32, 8, 4096, 40), ("self64_L32", 32, 8, 4096, 40)]
-ONLY = sys.argv[1] if len(sys.argv) > 1 else None   # e.g. `self64`: one shape, few iterations (ncu captures)
+ONLY = sys.argv[1] if len(sys.argv) > 1 else None   # e.g. `self64`: one shape, few iterations (profiler captures)
 for name, B, H, N, dh in shapes:
     if ONLY and name != ONLY:
         continue

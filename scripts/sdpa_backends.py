@@ -1,4 +1,4 @@
-"""Which library SDPA backend is fastest on B200 for the spatial attention shapes of the SD1.5 UNet (fwd and fwd+bwd)?"""
+"""Which library SDPA backend is fastest on the H100 for the spatial attention shapes of the SD1.5 UNet (fwd and fwd+bwd)?"""
 import torch, time
 from torch.nn.attention import sdpa_kernel, SDPBackend
 import torch.nn.functional as F

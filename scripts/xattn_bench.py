@@ -1,5 +1,5 @@
 """Microbenchmark of the text cross-attention core (reference models/attention.py:280-285 -> :535-542) at the four
-layer shapes of the SD1.5 UNet (16 x 512 x 512): this package's tcgen05 kernels (csrc/cross_attn_fwd_tc.cu, csrc/cross_attn_bwd_tc.cu) next to the
+layer shapes of the SD1.5 UNet (16 x 512 x 512): this package's wgmma kernels (csrc/spatial_attn_tc.cu, csrc/spatial_attn_bwd_tc.cu) next to the
 library kernel that F.scaled_dot_product_attention picks for the same strided views. CUDA events, L2 flushed between
 launches, 3 warm-ups, median of 20. One JSON line per shape. Algorithmic bytes: forward = Q read + O written;
 backward (dQ only: the text K/V carry no gradient, weights are frozen) = Q, dO read + dQ written."""

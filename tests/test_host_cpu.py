@@ -166,14 +166,14 @@ def test_linear_into_residual_accumulates_in_place_only_without_grad():
 
 
 def test_exp2_polynomial_coefficients_accuracy():
-    """csrc/tma_common.cuh ex2_poly_pair: the softmax kernels evaluate a quarter of their exponentials as
+    """csrc/tma_common.cuh ex2_poly: the softmax kernels evaluate a quarter of their exponentials as
     2^round(x) * poly(x - round(x)) on the FMA pipe. The coefficients are read from the source and the fp32 arithmetic is
     replayed in numpy: max relative error vs 2^x must stay far below the fp16 rounding (4.9e-4) applied right after."""
     import numpy as np
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     src = open(os.path.join(root, "motionclone_b200", "csrc", "tma_common.cuh")).read()
-    body = src[src.index("ex2_poly_pair("):src.index("MC_EX2_POLY_PERIOD")]
-    ks = {m.group(1): np.float32(m.group(2)) for m in re.finditer(r'"=l"\((k\d)\) : "f"\(([0-9.eE+-]+)f\)', body)}
+    body = src[src.index("ex2_poly("):src.index("MC_EX2_POLY_PERIOD")]
+    ks = {m.group(1): np.float32(m.group(2)) for m in re.finditer(r'constexpr float (k\d) = ([0-9.eE+-]+)f;', body)}
     assert sorted(ks) == ["k0", "k1", "k2", "k3", "k4"]
     x = np.concatenate([np.linspace(-126, 8.5, 400001), np.linspace(-1, 1, 100001)]).astype(np.float32)
     magic = np.float32(12582912.0)

@@ -413,7 +413,7 @@ def test_bias_residual_add():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# S2: text cross-attention on tcgen05 / TMEM
+# S2: text cross-attention on the wgmma attention kernels
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("B,Nq,Nk,H,DH", [(1, 256, 77, 8, 40), (2, 1024, 77, 8, 80), (1, 384, 77, 8, 160), (1, 128, 77, 2, 16),
                                           (1, 200, 77, 8, 32), (1, 4096, 77, 8, 40), (1, 128, 64, 8, 64)])

@@ -122,8 +122,7 @@ def test_motion_representation_vs_reference(run):
         # every index mismatch, in EVERY guided module, must sit on a row that is a near-tie in the REFERENCE's own fp32
         # probabilities (fixture key extract_top2gap_i = top-1 minus top-2 probability of the reference's rows). The
         # bound is an fp16 statement: q, k reach the softmax through ~100 fp16 layers, so two probabilities closer than
-        # the accumulated fp16 error of a score can legitimately swap order (measured on B200: every mismatching row has a
-        # reference gap <= 3.7e-3, i.e. <= 30 fp16 ulps of a probability ~ 1/L; the bar is 8e-3).
+        # the accumulated fp16 error of a score can legitimately swap order (8e-3 is ~64 fp16 ulps of a probability ~ 1/L).
         gap = torch.from_numpy(g[f"extract_top2gap_{i}"]).unsqueeze(-1)
         worst = float(gap[bad].max()) if bool(bad.any()) else 0.0
         worst_gaps.append(worst)

@@ -1,4 +1,4 @@
-"""Spatial self-attention (csrc/spatial_attn_tc.cu, tcgen05 + tensor-map TMA) through the C ABI against
+"""Spatial self-attention (csrc/spatial_attn_tc.cu, wgmma + tensor-map TMA) through the C ABI against
   (a) the math statement of the reference seam in fp64 (attention.py:461-490 on the same fp16 inputs), and
   (b) the library kernel the reference's xformers call maps to on this torch (F.scaled_dot_product_attention).
 Tolerance: fp16 output rounding (half an ulp of |o| <= 4 is 2e-3) plus fp16 rounding of the probabilities fed to P V.
@@ -62,7 +62,8 @@ def test_spatial_attention_forward(B, H, N, dh, fused):
 
 
 def test_spatial_attention_large_scores():
-    """Rows whose maximum jumps by far more than the lazy-rescale threshold between key tiles (O is rescaled in TMEM)."""
+    """Rows whose maximum jumps by orders of magnitude between key tiles: the online softmax must rescale the running
+    O and row sum (held in registers) by exp2(m_old - m_new) on every tile where the maximum grows."""
     dev = torch.device("cuda:0")
     B, H, N, dh = 1, 2, 512, 40
     C = H * dh
@@ -93,7 +94,7 @@ BWD_CASES = [(1, 8, 4096, 40), (2, 8, 1024, 80), (2, 8, 256, 160), (2, 8, 64, 16
 
 @pytest.mark.parametrize("B,H,N,dh", BWD_CASES)
 def test_spatial_attention_backward(B, H, N, dh):
-    """dQ, dK, dV of the tcgen05 backward against fp64 autograd of the math statement on the same fp16 inputs; the
+    """dQ, dK, dV of the wgmma backward against fp64 autograd of the math statement on the same fp16 inputs; the
     library kernel's own error against the same truth is the yardstick."""
     torch.manual_seed(N * 3 + dh)
     dev = torch.device("cuda:0")

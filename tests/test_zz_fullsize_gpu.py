@@ -62,7 +62,7 @@ def test_temporal_attention_full_size_position_permutation_and_top1():
 
 
 def test_cross_attention_full_size_row_permutation():
-    """attn2 on tcgen05 (models/attention.py:280-285 -> :535-542): 16 x 4096 query rows against the 77 text keys."""
+    """attn2 on the wgmma kernels (models/attention.py:280-285 -> :535-542): 16 x 4096 query rows against the 77 text keys."""
     ops, dev = _ops(), _dev()
     g = torch.Generator().manual_seed(12)
     nq = L * D

@@ -14,9 +14,11 @@
 // and D = sum_j P_j dP_j computed in place (exact, no statistics from the forward).
 // Every streamed [rows][DH] tile serves two GEMMs through two descriptors - K-major where DH is contracted (S, dP),
 // MN-major where the rows are (dS K, P^T dO, dS^T Q) - so nothing is transposed or copied twice; the tiles the threads
-// produce (P^T, dS, dS^T) are register A operands of the next wgmma and never touch shared memory. There are no masks in
-// the spatial kernels: rows past the end of the sequence are zero-filled by the TMA unit, and a zero K / V / Q / dO row
-// contributes nothing to any of the sums (the padded statistics keep every intermediate finite). The two-kernel split
+// produce (P^T, dS, dS^T) are register A operands of the next wgmma and never touch shared memory. Rows past the end of
+// the sequence are zero-filled by the TMA unit. In the dK/dV kernel a padded query row needs no mask: its statistics are
+// padded with lse2 = Dsc = 0, so P^T = 1 and dS^T = 0 stay finite, and its zero Q / dO row adds nothing. The dQ kernel
+// scores a padded KEY against a real row's statistics, P = exp(-lse), which overflows for very negative lse: it zeroes
+// dS of the keys past the end of the last tile, as the forward and the SINGLE path mask them to -inf. The two-kernel split
 // recomputes S and dP once more than a fused kernel would but needs no atomics on dQ: results are deterministic.
 #include <math.h>
 
@@ -105,7 +107,9 @@ struct DQCfg {
 
 // dQ for 128 queries: warpgroups 0, 1 own 64 rows each; warp 8 lane 0 issues the TMA loads (Q and dO resident, K and V
 // streamed). SINGLE: the whole key axis (<= kMaxTextKeys) is one tile and the softmax statistics are computed here.
-template <int DH, bool SINGLE>
+// RAGGED (spatial only, launched when Nk % 64 != 0): dS of the keys past the end of the last tile is zeroed; a separate
+// instantiation so that the 64-aligned token counts run the unmasked code unchanged.
+template <int DH, bool SINGLE, bool RAGGED>
 __global__ void __launch_bounds__(DQCfg<DH, SINGLE>::THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap mq128, const __grid_constant__ CUtensorMap mq32,
                    const __grid_constant__ CUtensorMap mdo128, const __grid_constant__ CUtensorMap mdo32,
@@ -232,6 +236,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap mq128, const __grid_const
         const int r = (i >> 1) & 1;
         const float p = ex2_approx(fmaf(s[i], c, neg_lse2[r]));
         dp[i] = p * fmaf(dp[i], scale, -dscr[r]);
+      }
+      if constexpr (RAGGED) {
+        // Keys past the end of the sequence: the zero-filled K row scores s = 0 against this row's statistics, so
+        // p = exp(-lse) overflows fp16 (or fp32) when lse is very negative, and inf x 0 in dS K would be NaN.
+        const int kvalid = prm.Nk - j * BN;
+        if (kvalid < BN) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i)
+            if ((i >> 2) * 8 + 2 * t + (i & 1) >= kvalid) dp[i] = 0.f;
+        }
       }
     }
     uint32_t da[BN / 4];
@@ -364,7 +378,10 @@ template <int DH, bool SINGLE>
 static int launch_dq(const AttnMaps& q, const AttnMaps& d_o, const AttnMaps& k, const AttnMaps& v, const FABwdParams& prm,
                      cudaStream_t st) {
   using X = DQCfg<DH, SINGLE>;
-  auto kern = attn_bwd_dq_kernel<DH, SINGLE>;
+  auto kern = attn_bwd_dq_kernel<DH, SINGLE, false>;
+  if constexpr (!SINGLE) {
+    if (prm.Nk % kBT) kern = attn_bwd_dq_kernel<DH, false, true>;
+  }
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, X::SMEM);
   dim3 grid((prm.Nq + kBM - 1) / kBM, prm.H, prm.B);
   kern<<<grid, X::THREADS, X::SMEM, st>>>(q.m128, q.m32, d_o.m128, d_o.m32, k.m128, k.m32, v.m128, v.m32, prm);

@@ -27,7 +27,7 @@ from torch import nn
 from . import ops
 
 
-_XATTN_TC_HEAD_DIMS = (8, 16, 32, 40, 64, 80, 160)  # instantiations of csrc/cross_attn_{fwd,bwd}_tc.cu
+_XATTN_TC_HEAD_DIMS = (8, 16, 32, 40, 64, 80, 160)  # instantiations of csrc/spatial_attn_tc.cu, csrc/spatial_attn_bwd_tc.cu
 
 
 def _need_kernels(x, what: str) -> None:

@@ -57,7 +57,9 @@ void mc_add_launch_count(uint64_t n);
  *   top_val/top_idx [B*D, H, L]    : torch.topk(k=1) + uint8 cast, utils/motionclone_functions.py:79 (ties: lowest index)
  *   gathered   [B*D, H, L] fp16    : torch.gather(P, idx_ref), utils/motionclone_functions.py:91-92
  * Any of o, probs, top_val/top_idx, gather_idx/gathered may be NULL (v may be NULL iff o is NULL).
- * L in {8, 16, 32} (positional encoding max_len is 32, models/motion_module.py:60); DH in {8,16,32,40,64,80,128,160}.
+ * L in 1..32 (positional encoding max_len is 32, models/motion_module.py:60; other values return MC_E_UNSUPPORTED);
+ * DH in {8,16,32,40,64,80,128,160}. Lengths other than 8, 16, 32 run in the next larger of those tiles with the padded
+ * frames masked; every per-row tensor has exactly L entries per row (row stride L).
  */
 int mc_temporal_attn_fwd(const void* q, const void* k, const void* v, mc_temporal_layout qkv_layout,
                          void* o, mc_temporal_layout o_layout,
@@ -73,7 +75,7 @@ int mc_temporal_attn_fwd(const void* q, const void* k, const void* v, mc_tempora
  *   d_probs    : dense gradient of probs [B*D, H, L, L] fp16
  *   gather_idx + d_gathered [B*D, H, L] : one-hot gradient of the gathered probabilities (closed form of
  *                gather + mse_loss backward, utils/motionclone_functions.py:92-96)
- * Outputs dq, dk (and dv unless NULL) share g_layout.
+ * Outputs dq, dk (and dv unless NULL) share g_layout. L in 1..32, as for the forward.
  */
 int mc_temporal_attn_bwd(const void* q, const void* k, const void* v, mc_temporal_layout qkv_layout,
                          const void* d_o, mc_temporal_layout do_layout,
@@ -82,7 +84,7 @@ int mc_temporal_attn_bwd(const void* q, const void* k, const void* v, mc_tempora
                          int B, int D, int L, int H, int DH, float scale, void* stream);
 
 /* torch.topk(k=1, dim=-1) over fp16 rows of length L (utils/motionclone_functions.py:79); rows = product of the
- * leading dims. Stand-alone form of the fused epilogue above. */
+ * leading dims, L in 1..32. Stand-alone form of the fused epilogue above. */
 int mc_top1_rows(const void* probs, int64_t rows, int L, void* top_val, uint8_t* top_idx, void* stream);
 
 /*

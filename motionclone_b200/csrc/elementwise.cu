@@ -128,6 +128,26 @@ __global__ void __launch_bounds__(256) top1_rows_kernel(const __half* __restrict
   }
 }
 
+// top-1 of fp16 rows of any other length L <= 32: one thread per row and 2-byte loads, since a row starts at row*L
+// halves (any alignment); lowest index wins ties
+__global__ void __launch_bounds__(256) top1_rows_any_kernel(const __half* __restrict__ probs, int64_t rows, int L,
+                                                            __half* __restrict__ val, uint8_t* __restrict__ idx) {
+  const int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (row >= rows) return;
+  const __half* p = probs + row * L;
+  float bv = -1.f;
+  int bi = 0;
+  for (int j = 0; j < L; ++j) {
+    const float v = __half2float(__ldg(p + j));
+    if (v > bv) {
+      bv = v;
+      bi = j;
+    }
+  }
+  val[row] = __float2half_rn(bv);
+  idx[row] = (uint8_t)bi;
+}
+
 // out = a + b + bias[c] on channel-innermost (NHWC / token-major) fp16 tensors: the resnet's `input + conv2(...)`
 // (models/resnet.py:209-211) with conv2's (and the shortcut conv's) bias folded in, one pass instead of three.
 // Rounding: the eager graph rounds conv+bias to fp16, then the sum; here h(h(a + bias) + b).
@@ -281,7 +301,11 @@ extern "C" int mc_top1_rows(const void* probs, int64_t rows, int L, void* top_va
     set_error("top1_rows: null pointer or rows <= 0");
     return MC_E_INVALID;
   }
-  const int lpr = L / 8;
+  if (L < 1 || L > 32) {
+    set_error("top1_rows: L=%d outside the supported range 1..32", L);
+    return MC_E_UNSUPPORTED;
+  }
+  const int lpr = (L == 8 || L == 16 || L == 32) ? L / 8 : 1;  // lanes per row
   const int64_t threads = rows * lpr;
   const unsigned grid = (unsigned)((threads + 255) / 256);
   cudaStream_t st = (cudaStream_t)stream;
@@ -291,10 +315,8 @@ extern "C" int mc_top1_rows(const void* probs, int64_t rows, int L, void* top_va
     top1_rows_kernel<16><<<grid, 256, 0, st>>>((const __half*)probs, rows, (__half*)top_val, top_idx);
   else if (L == 32)
     top1_rows_kernel<32><<<grid, 256, 0, st>>>((const __half*)probs, rows, (__half*)top_val, top_idx);
-  else {
-    set_error("top1_rows: L=%d unsupported (8, 16, 32)", L);
-    return MC_E_UNSUPPORTED;
-  }
+  else
+    top1_rows_any_kernel<<<grid, 256, 0, st>>>((const __half*)probs, rows, L, (__half*)top_val, top_idx);
   count_launch();
   return check_launch("top1_rows");
 }

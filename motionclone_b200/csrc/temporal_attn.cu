@@ -4,7 +4,7 @@
 // second softmax pass of get_temp_attn_prob (utils/motionclone_functions.py:260-283 -> models/attention.py:564-611),
 // torch.topk(k=1) (utils/motionclone_functions.py:79) and torch.gather (…:92) — one pass over Q, K, V.
 //
-// Shape of the problem: per (batch, position, head) a 16x16 (L x L, L in {8,16,32}) attention with DH in [8,160]:
+// Shape of the problem: per (batch, position, head) a 16x16 (L x L, L in 1..32) attention with DH in [8,160]:
 // arithmetic intensity L/2 flop/byte => HBM-bound (DESIGN.md §4, T1/T2). One CTA stages a tile of
 // (all L frames) x (P positions) x (HG heads) of Q, K, V in shared memory with 1-D bulk copies (TMA engine, UBLKCP)
 // signalled on mbarriers; each warp owns (position, head) items: QK^T, the fp16-rounded softmax and PV run on
@@ -14,6 +14,11 @@
 //
 // The frame pitch in shared memory is padded to 16 (mod 128) bytes so the 8 row addresses of every ldmatrix phase
 // fall in 8 different 16 B bank groups (rows of one (position, head) item are `pitch` apart).
+//
+// Clip lengths other than 8, 16 and 32 frames run "ragged" in the next larger tile (LP = 8 for L <= 8, 16 for L <= 16,
+// 32 otherwise), in separate instantiations (RAGGED = true) so the tile lengths themselves keep their machine code:
+// only frames 0..L-1 are copied in and out, frames L..LP-1 of every staged tile are zero-filled, key columns >= L are
+// left out of the softmax (probability exactly 0) and no per-row output or input is touched for a frame >= L.
 #include <math.h>
 #include <stdlib.h>
 
@@ -21,8 +26,9 @@
 
 #include "mc_common.cuh"
 
-// The file can be compiled as two translation units (build time): -DMC_TA_PART=1 keeps the forward entry point and its
-// instantiations, =2 the backward ones; undefined / 0 keeps both.
+// The file can be compiled as four translation units (build time): -DMC_TA_PART=1 keeps the forward entry point and its
+// tile-length instantiations, =2 the backward ones, =3 / =4 the ragged forward / backward instantiations; undefined / 0
+// keeps everything.
 #ifndef MC_TA_PART
 #define MC_TA_PART 0
 #endif
@@ -31,10 +37,12 @@ namespace mc {
 
 constexpr int kHeaderBytes = 128;
 
-template <int DH_, int L_>
+// L is the tile length (8, 16 or 32). RAGGED: the clip has fewer frames than the tile (TAParams::L at run time).
+template <int DH_, int L_, bool RAGGED_ = false>
 struct TACfg {
   static constexpr int DH = DH_;
   static constexpr int L = L_;
+  static constexpr bool RAGGED = RAGGED_;
   static constexpr int MT = (L + 15) / 16;           // 16-row query tiles per item
   static constexpr int NKT = (L == 8) ? 2 : L / 8;   // 8-wide key tiles in the score fragment
   static constexpr int KK = (L == 8) ? 1 : L / 16;   // k16 steps over keys (P V, dS K, ...)
@@ -84,6 +92,7 @@ struct TAParams {
   int B, D, H;
   TileGeom g;
   float scale;
+  int L;                      // frames of the clip (<= the tile length; read by the ragged instantiations only)
 };
 
 // Byte offset (inside one staged tensor) of "virtual row" idx of an item whose first position is pl0.
@@ -105,11 +114,11 @@ __device__ __forceinline__ uint32_t xrow_off(int idx, int pl0, const G& g) {
 // Stage `ntensors` tensors (same layout) of this CTA's tile: rows of W halfs per (frame, position).
 // rows of `w` halfs per (frame, position); smem: frame pitch `spitch` bytes, position stride `sps` halfs.
 // When positions are contiguous on both sides (global stride_p == w == sps) one copy per frame moves all P of them.
-template <int L>
-__device__ __forceinline__ void stage_rows(uint8_t* sdst, int spitch, int sps, int w, int P, const __half* gsrc,
+// `nf`: frames 0..nf-1 are copied (the clip length; a compile-time constant outside the ragged instantiations).
+__device__ __forceinline__ void stage_rows(int nf, uint8_t* sdst, int spitch, int sps, int w, int P, const __half* gsrc,
                                            const mc_temporal_layout& lay, int64_t gbase, uint64_t* bar, int lane) {
   const bool merged = (lay.stride_p == w) && (sps == w);
-  const int ncopies = merged ? L : L * P;
+  const int ncopies = merged ? nf : nf * P;
   const uint32_t bytes = (merged ? P : 1) * w * 2;
   for (int i = lane; i < ncopies; i += 32) {
     const int f = merged ? i : i / P;
@@ -118,16 +127,26 @@ __device__ __forceinline__ void stage_rows(uint8_t* sdst, int spitch, int sps, i
   }
 }
 
-template <int L>
-__device__ __forceinline__ void store_rows(__half* gdst, const uint8_t* ssrc, int spitch, int sps, int w, int P,
+__device__ __forceinline__ void store_rows(int nf, __half* gdst, const uint8_t* ssrc, int spitch, int sps, int w, int P,
                                            const mc_temporal_layout& lay, int64_t gbase, int lane) {
   const bool merged = (lay.stride_p == w) && (sps == w);
-  const int ncopies = merged ? L : L * P;
+  const int ncopies = merged ? nf : nf * P;
   const uint32_t bytes = (merged ? P : 1) * w * 2;
   for (int i = lane; i < ncopies; i += 32) {
     const int f = merged ? i : i / P;
     const int pl = merged ? 0 : i % P;
     bulk_s2g(gdst + gbase + f * lay.stride_f + pl * lay.stride_p, ssrc + f * spitch + pl * sps * 2, bytes);
+  }
+}
+
+// Ragged tiles: zero frames nf..L-1 of `ntiles` staged tiles (`stride` bytes apart, frames `pitch` bytes apart) with
+// ordinary stores, so that the padded rows and key columns hold zeros rather than whatever shared memory held before
+// (a NaN pattern there would survive 0 * NaN in P V). Every thread of the CTA takes part.
+__device__ __forceinline__ void zero_frames(uint8_t* base, int ntiles, int stride, int pitch, int nf, int L) {
+  const int chunks = (L - nf) * pitch / 16;  // pitch is a multiple of 16 bytes
+  for (int i = threadIdx.x; i < ntiles * chunks; i += blockDim.x) {
+    const int tile = i / chunks, c = i % chunks;
+    *reinterpret_cast<uint4*>(base + tile * stride + nf * pitch + c * 16) = make_uint4(0u, 0u, 0u, 0u);
   }
 }
 
@@ -178,19 +197,29 @@ __device__ __forceinline__ void qk_scores(float (&s)[C::NKT][4], uint32_t sQ, ui
 // In place: s <- fp16-rounded probabilities (as fp32 values). Rounding points follow models/attention.py:466-483:
 // scores -> fp16 (baddbmm output), softmax in fp32 with the butterfly summation order of ATen's warp softmax,
 // probabilities -> fp16.
+// Ragged tiles (nf < L keys): key columns >= nf are left out of the row max and contribute an exact +0 to the sum, so
+// the summation tree over L columns gives the same partial sums as ATen's warp softmax over nf columns, which pads a
+// row to next_pow2(nf) lanes with -inf (exp -> 0) and reduces with xor offsets from the largest down.
 template <typename C>
-__device__ __forceinline__ void softmax_rows(float (&s)[C::NKT][4], float scale) {
+__device__ __forceinline__ bool key_valid(int nt, int hf, int e, int t, int nf) {
+  const bool in_tile = (C::L != 8) || (nt == hf);
+  return in_tile && (!C::RAGGED || (C::L == 8 ? 0 : nt * 8) + 2 * t + e < nf);
+}
+
+template <typename C>
+__device__ __forceinline__ void softmax_rows(float (&s)[C::NKT][4], float scale, int nf, int lane) {
+  const int t = lane & 3;
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     float x[C::NKT][2];
     float mx = -INFINITY;
 #pragma unroll
     for (int nt = 0; nt < C::NKT; ++nt) {
-      const bool valid = (C::L != 8) || (nt == hf);
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         x[nt][e] = round_half(s[nt][2 * hf + e] * scale);
-        if (valid) mx = fmaxf(mx, x[nt][e]);
+        if (C::RAGGED && !key_valid<C>(nt, hf, e, t, nf)) x[nt][e] = -INFINITY;  // exp -> exactly +0
+        if (key_valid<C>(nt, hf, e, t, nf)) mx = fmaxf(mx, x[nt][e]);
       }
     }
     mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
@@ -219,12 +248,11 @@ __device__ __forceinline__ void softmax_rows(float (&s)[C::NKT][4], float scale)
     const float y = __frcp_rn(sum);
 #pragma unroll
     for (int nt = 0; nt < C::NKT; ++nt) {
-      const bool valid = (C::L != 8) || (nt == hf);
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const float q0 = x[nt][e] * y;
         const float q1 = fmaf(fmaf(-q0, sum, x[nt][e]), y, q0);
-        s[nt][2 * hf + e] = valid ? round_half(q1) : 0.f;
+        s[nt][2 * hf + e] = key_valid<C>(nt, hf, e, t, nf) ? round_half(q1) : 0.f;
       }
     }
   }
@@ -280,12 +308,18 @@ __device__ __forceinline__ void probs_to_afrag(uint32_t (&pa)[C::KK][4], const f
   }
 }
 
-// row bookkeeping of an item: global row index R = ((b*D + pos)*H + h)*L + frame for accumulator half hf of tile mt
+// row bookkeeping of an item: global row index R = ((b*D + pos)*H + h)*nf + frame for accumulator half hf of tile mt
+// (nf: frames of the clip, the row stride of every per-row tensor)
 template <typename C>
 __device__ __forceinline__ int64_t out_row(int b, int p_first, int p_last, int h, int mt, int gq, int hf, int D,
-                                           int H) {
-  if (C::L == 8) return ((int64_t)(b * D + min(p_first + hf, p_last)) * H + h) * 8 + gq;
-  return ((int64_t)(b * D + p_first) * H + h) * C::L + mt * 16 + gq + 8 * hf;
+                                           int H, int nf) {
+  if (C::L == 8) return ((int64_t)(b * D + min(p_first + hf, p_last)) * H + h) * nf + gq;
+  return ((int64_t)(b * D + p_first) * H + h) * nf + mt * 16 + gq + 8 * hf;
+}
+// frame of that row; a ragged tile's rows at frames >= nf are padding and neither load nor store per-row data
+template <typename C>
+__device__ __forceinline__ int row_frame(int mt, int gq, int hf) {
+  return C::L == 8 ? gq : mt * 16 + gq + 8 * hf;
 }
 
 // ================================================================================================================
@@ -296,7 +330,7 @@ __device__ __forceinline__ int64_t out_row(int b, int p_first, int p_last, int h
 template <typename C, typename G>
 __device__ __forceinline__ void fwd_item(const TAParams& prm, const G& g, uint8_t* sQ, uint32_t sQa, uint32_t sKa,
                                          uint32_t sVa, int b, int p0, int h0, int item, int lane, bool has_o,
-                                         uint64_t* bar_v, bool& v_ready) {
+                                         uint64_t* bar_v, bool& v_ready, int nf) {
   constexpr int DH = C::DH;
   constexpr int L = C::L;
   const int gq = lane >> 2, t = lane & 3;
@@ -308,19 +342,25 @@ __device__ __forceinline__ void fwd_item(const TAParams& prm, const G& g, uint8_
   for (int mt = 0; mt < C::MT; ++mt) {
     float s[C::NKT][4];
     qk_scores<C>(s, sQa, sKa, mt, pl0, colbase, g, lane);
-    softmax_rows<C>(s, prm.scale);
+    softmax_rows<C>(s, prm.scale, nf, lane);
 
     // ---- per-row outputs: probabilities, top-1 (lowest index on ties), gathered probability ----
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
-      const int64_t R = out_row<C>(b, p0 + pl0, p0 + g.P - 1, h, mt, gq, hf, prm.D, prm.H);
-      if (prm.probs != nullptr) {
-        __half* prow = prm.probs + R * L;
+      const int64_t R = out_row<C>(b, p0 + pl0, p0 + g.P - 1, h, mt, gq, hf, prm.D, prm.H, nf);
+      const bool row_ok = !C::RAGGED || row_frame<C>(mt, gq, hf) < nf;
+      if (prm.probs != nullptr && row_ok) {
+        __half* prow = prm.probs + R * nf;
 #pragma unroll
         for (int nt = 0; nt < C::NKT; ++nt) {
           if (L == 8 && nt != hf) continue;
           const int col = (L == 8 ? 0 : nt * 8) + 2 * t;
-          *reinterpret_cast<__half2*>(prow + col) = __floats2half2_rn(s[nt][2 * hf], s[nt][2 * hf + 1]);
+          if (C::RAGGED) {  // row R starts at R*nf halves: any parity, so 2-byte stores only
+            if (col < nf) prow[col] = __float2half_rn(s[nt][2 * hf]);
+            if (col + 1 < nf) prow[col + 1] = __float2half_rn(s[nt][2 * hf + 1]);
+          } else {
+            *reinterpret_cast<__half2*>(prow + col) = __floats2half2_rn(s[nt][2 * hf], s[nt][2 * hf + 1]);
+          }
         }
       }
       if (prm.top_val != nullptr) {
@@ -333,6 +373,7 @@ __device__ __forceinline__ void fwd_item(const TAParams& prm, const G& g, uint8_
           for (int e = 0; e < 2; ++e) {
             const float pv = s[nt][2 * hf + e];
             const int col = (L == 8 ? 0 : nt * 8) + 2 * t + e;
+            if (C::RAGGED && col >= nf) continue;
             if (pv > bv) {
               bv = pv;
               bi = col;
@@ -348,12 +389,12 @@ __device__ __forceinline__ void fwd_item(const TAParams& prm, const G& g, uint8_
             bi = oi;
           }
         }
-        if (t == 0) {
+        if (t == 0 && row_ok) {
           prm.top_val[R] = __float2half_rn(bv);
           prm.top_idx[R] = (uint8_t)bi;
         }
       }
-      if (prm.gathered != nullptr) {
+      if (prm.gathered != nullptr && row_ok) {
         const int gi = prm.gather_idx[R];
 #pragma unroll
         for (int nt = 0; nt < C::NKT; ++nt) {
@@ -396,13 +437,14 @@ __device__ __forceinline__ G load_geom(const TAParams& prm) {
   }
 }
 
-template <int DH, int L, int NW, typename G = TileGeom>
+template <int DH, int L, int NW, typename G = TileGeom, bool RAGGED = false>
 __global__ void __launch_bounds__(NW * 32) temporal_attn_fwd_kernel(const TAParams prm) {
-  using C = TACfg<DH, L>;
+  using C = TACfg<DH, L, RAGGED>;
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* bar_qk = reinterpret_cast<uint64_t*>(smem);
   uint64_t* bar_v = bar_qk + 1;
   const G g = load_geom<G>(prm);
+  const int nf = RAGGED ? prm.L : L;  // frames of the clip
   uint8_t* sQ = smem + kHeaderBytes;
   uint8_t* sK = g.fused ? sQ + g.W * 2 : sQ + g.tensor_bytes;       // fused: K, V are column offsets of one tile
   uint8_t* sV = g.fused ? sQ + g.W * 4 : sQ + 2 * g.tensor_bytes;
@@ -422,23 +464,24 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_fwd_kernel(const TAPara
     mbar_init(bar_v, 1);
     fence_mbar_init();
   }
+  if (RAGGED) zero_frames(sQ, g.fused ? 1 : 3, g.tensor_bytes, g.pitch, nf, L);
   __syncthreads();
   if (warp == 0) {
-    const uint32_t tbytes = (uint32_t)L * g.P * g.W * 2;
+    const uint32_t tbytes = (uint32_t)nf * g.P * g.W * 2;  // exactly the bytes the copies below bring in
     const int64_t gbase = (int64_t)b * prm.in.stride_b + (int64_t)p0 * prm.in.stride_p + h0 * DH;
     if (g.fused) {
       if (lane == 0) mbar_arrive_expect_tx(bar_qk, 3 * tbytes);
       __syncwarp();
-      stage_rows<L>(sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
+      stage_rows(nf, sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
     } else {
       if (lane == 0) {
         mbar_arrive_expect_tx(bar_qk, 2 * tbytes);
         if (has_o) mbar_arrive_expect_tx(bar_v, tbytes);
       }
       __syncwarp();
-      stage_rows<L>(sQ, g.pitch, g.PS, g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
-      stage_rows<L>(sK, g.pitch, g.PS, g.W, g.P, prm.k, prm.in, gbase, bar_qk, lane);
-      if (has_o) stage_rows<L>(sV, g.pitch, g.PS, g.W, g.P, prm.v, prm.in, gbase, bar_v, lane);
+      stage_rows(nf, sQ, g.pitch, g.PS, g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
+      stage_rows(nf, sK, g.pitch, g.PS, g.W, g.P, prm.k, prm.in, gbase, bar_qk, lane);
+      if (has_o) stage_rows(nf, sV, g.pitch, g.PS, g.W, g.P, prm.v, prm.in, gbase, bar_v, lane);
     }
   }
   mbar_wait(bar_qk, 0);
@@ -448,14 +491,14 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_fwd_kernel(const TAPara
   bool v_ready = false;
 
   for (int item = warp; item < n_items; item += NW)
-    fwd_item<C>(prm, g, sQ, sQa, sKa, sVa, b, p0, h0, item, lane, has_o, g.fused ? nullptr : bar_v, v_ready);
+    fwd_item<C>(prm, g, sQ, sQa, sKa, sVa, b, p0, h0, item, lane, has_o, g.fused ? nullptr : bar_v, v_ready, nf);
 
   if (has_o) {
     fence_proxy_async();
     __syncthreads();
     if (warp == 0) {
       const int64_t obase = (int64_t)b * prm.out.stride_b + (int64_t)p0 * prm.out.stride_p + h0 * DH;
-      store_rows<L>(prm.o, sQ, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
+      store_rows(nf, prm.o, sQ, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
       bulk_commit();
       bulk_wait_read_all();
     }
@@ -466,14 +509,15 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_fwd_kernel(const TAPara
 // backward: dq, dk, dv from d_o and/or the probability branches. Staged: Q, K, V, dO; outputs reuse dead tiles
 // (dV -> V, dQ -> dO, dK -> K).
 // ================================================================================================================
-template <int DH, int L, int NW, typename G = TileGeom>
+template <int DH, int L, int NW, typename G = TileGeom, bool RAGGED = false>
 __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAParams prm) {
-  using C = TACfg<DH, L>;
+  using C = TACfg<DH, L, RAGGED>;
   static_assert(C::MT == 1 || L == 32, "");
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* bar_qk = reinterpret_cast<uint64_t*>(smem);
   uint64_t* bar_v = bar_qk + 1;
   const G g = load_geom<G>(prm);
+  const int nf = RAGGED ? prm.L : L;  // frames of the clip
   uint8_t* sQ = smem + kHeaderBytes;
   uint8_t* sK = g.fused ? sQ + g.W * 2 : sQ + g.tensor_bytes;
   uint8_t* sV = g.fused ? sQ + g.W * 4 : sQ + 2 * g.tensor_bytes;
@@ -497,9 +541,13 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
     mbar_init(bar_v, 1);
     fence_mbar_init();
   }
+  if (RAGGED) {
+    zero_frames(sQ, g.fused ? 1 : 3, g.tensor_bytes, g.pitch, nf, L);
+    zero_frames(sD, 1, 0, g.pitch_x, nf, L);  // zero dO rows: padded queries add nothing to dV = P^T dO
+  }
   __syncthreads();
   if (warp == 0) {
-    const uint32_t tbytes = (uint32_t)L * g.P * g.W * 2;
+    const uint32_t tbytes = (uint32_t)nf * g.P * g.W * 2;  // exactly the bytes the copies below bring in
     const int64_t gbase = (int64_t)b * prm.in.stride_b + (int64_t)p0 * prm.in.stride_p + h0 * DH;
     const int64_t dbase = (int64_t)b * prm.dol.stride_b + (int64_t)p0 * prm.dol.stride_p + h0 * DH;
     if (g.fused) {
@@ -508,19 +556,19 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
         if (has_do) mbar_arrive_expect_tx(bar_v, tbytes);
       }
       __syncwarp();
-      stage_rows<L>(sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
-      if (has_do) stage_rows<L>(sD, g.pitch_x, g.W, g.W, g.P, prm.d_o, prm.dol, dbase, bar_v, lane);
+      stage_rows(nf, sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
+      if (has_do) stage_rows(nf, sD, g.pitch_x, g.W, g.W, g.P, prm.d_o, prm.dol, dbase, bar_v, lane);
     } else {
       if (lane == 0) {
         mbar_arrive_expect_tx(bar_qk, 2 * tbytes);
         if (has_do) mbar_arrive_expect_tx(bar_v, 2 * tbytes);
       }
       __syncwarp();
-      stage_rows<L>(sQ, g.pitch, g.PS, g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
-      stage_rows<L>(sK, g.pitch, g.PS, g.W, g.P, prm.k, prm.in, gbase, bar_qk, lane);
+      stage_rows(nf, sQ, g.pitch, g.PS, g.W, g.P, prm.q, prm.in, gbase, bar_qk, lane);
+      stage_rows(nf, sK, g.pitch, g.PS, g.W, g.P, prm.k, prm.in, gbase, bar_qk, lane);
       if (has_do) {
-        stage_rows<L>(sV, g.pitch, g.PS, g.W, g.P, prm.v, prm.in, gbase, bar_v, lane);
-        stage_rows<L>(sD, g.pitch_x, g.W, g.W, g.P, prm.d_o, prm.dol, dbase, bar_v, lane);
+        stage_rows(nf, sV, g.pitch, g.PS, g.W, g.P, prm.v, prm.in, gbase, bar_v, lane);
+        stage_rows(nf, sD, g.pitch_x, g.W, g.W, g.P, prm.d_o, prm.dol, dbase, bar_v, lane);
       }
     }
   }
@@ -544,7 +592,7 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
     for (int mt = 0; mt < C::MT; ++mt) {
       float p[C::NKT][4];
       qk_scores<C>(p, sQa, sKa, mt, pl0, colbase, g, lane);
-      softmax_rows<C>(p, prm.scale);
+      softmax_rows<C>(p, prm.scale, nf, lane);
       probs_to_afrag<C>(pfrag[mt], p);
 
       // dP = dO V^T  (+ dense d_probs, + one-hot d_gathered)
@@ -563,10 +611,11 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
       }
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        const int64_t R = out_row<C>(b, p0 + pl0, p0 + g.P - 1, h, mt, gq, hf, prm.D, prm.H);
+        const int64_t R = out_row<C>(b, p0 + pl0, p0 + g.P - 1, h, mt, gq, hf, prm.D, prm.H, nf);
+        const bool row_ok = !C::RAGGED || row_frame<C>(mt, gq, hf) < nf;
         int gi = -1;
         float gv = 0.f;
-        if (prm.d_gathered != nullptr) {
+        if (prm.d_gathered != nullptr && row_ok) {
           gi = prm.gather_idx[R];
           gv = __half2float(prm.d_gathered[R]);
         }
@@ -575,10 +624,16 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
         for (int nt = 0; nt < C::NKT; ++nt) {
           if (L == 8 && nt != hf) continue;
           const int col0 = (L == 8 ? 0 : nt * 8) + 2 * t;
-          if (prm.d_probs != nullptr) {
-            const __half2 dd = *reinterpret_cast<const __half2*>(prm.d_probs + R * L + col0);
-            dp[nt][2 * hf] += __low2float(dd);
-            dp[nt][2 * hf + 1] += __high2float(dd);
+          if (prm.d_probs != nullptr && row_ok) {
+            if (C::RAGGED) {  // row R starts at R*nf halves: any parity, so 2-byte loads, columns < nf only
+              const __half* drow = prm.d_probs + R * nf;
+              if (col0 < nf) dp[nt][2 * hf] += __half2float(drow[col0]);
+              if (col0 + 1 < nf) dp[nt][2 * hf + 1] += __half2float(drow[col0 + 1]);
+            } else {
+              const __half2 dd = *reinterpret_cast<const __half2*>(prm.d_probs + R * L + col0);
+              dp[nt][2 * hf] += __low2float(dd);
+              dp[nt][2 * hf + 1] += __high2float(dd);
+            }
           }
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
@@ -673,13 +728,13 @@ __global__ void __launch_bounds__(NW * 32) temporal_attn_bwd_kernel(const TAPara
   if (warp == 0) {
     const int64_t obase = (int64_t)b * prm.out.stride_b + (int64_t)p0 * prm.out.stride_p + h0 * DH;
     if (fused_out && (prm.dv != nullptr && has_do)) {
-      store_rows<L>(prm.dq, sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.out, obase, lane);  // dQ | dK | dV per frame
+      store_rows(nf, prm.dq, sQ, g.pitch, g.PS, 3 * g.W, g.P, prm.out, obase, lane);  // dQ | dK | dV per frame
     } else if (fused_out) {  // no dV: two column blocks per (frame, position)
-      store_rows<L>(prm.dq, sQ, g.pitch, g.PS, 2 * g.W, g.P, prm.out, obase, lane);
+      store_rows(nf, prm.dq, sQ, g.pitch, g.PS, 2 * g.W, g.P, prm.out, obase, lane);
     } else {
-      store_rows<L>(prm.dq, sD, g.pitch_x, g.W, g.W, g.P, prm.out, obase, lane);
-      store_rows<L>(prm.dk, sK, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
-      if (has_do && prm.dv != nullptr) store_rows<L>(prm.dv, sV, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
+      store_rows(nf, prm.dq, sD, g.pitch_x, g.W, g.W, g.P, prm.out, obase, lane);
+      store_rows(nf, prm.dk, sK, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
+      if (has_do && prm.dv != nullptr) store_rows(nf, prm.dv, sV, g.pitch, g.PS, g.W, g.P, prm.out, obase, lane);
     }
     bulk_commit();
     bulk_wait_read_all();
@@ -795,19 +850,22 @@ static bool try_launch_cgeom(const TAParams& prm, unsigned grid, int smem, int n
   return false;
 }
 
-template <int DH, int L>
+// L: the tile length; RAGGED: the clip has prm.L < L frames (runtime TileGeom only)
+template <int DH, int L, bool RAGGED = false>
 static int launch_fwd(TAParams& prm, cudaStream_t st) {
   choose_geom(prm.D, L, prm.H, DH, 3, L == 8, is_fusable(prm, prm.H * DH) && prm.o != nullptr, &prm.g, prm.B);
   const int smem = tile_smem(prm.g, 3);
   const int64_t grid = (int64_t)prm.B * (prm.D / prm.g.P) * (prm.H / prm.g.HG);
   const int n_items = ((prm.g.P + TACfg<DH, L>::PP - 1) / TACfg<DH, L>::PP) * prm.g.HG;
-  if (try_launch_cgeom<DH, L, false>(prm, (unsigned)grid, smem, n_items, st)) {
+  bool launched = false;
+  if constexpr (!RAGGED) launched = try_launch_cgeom<DH, L, false>(prm, (unsigned)grid, smem, n_items, st);
+  if (launched) {
   } else if (n_items >= 16) {
-    auto kern = temporal_attn_fwd_kernel<DH, L, 8>;
+    auto kern = temporal_attn_fwd_kernel<DH, L, 8, TileGeom, RAGGED>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     kern<<<(unsigned)grid, 8 * 32, smem, st>>>(prm);
   } else {
-    auto kern = temporal_attn_fwd_kernel<DH, L, 4>;
+    auto kern = temporal_attn_fwd_kernel<DH, L, 4, TileGeom, RAGGED>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     kern<<<(unsigned)grid, 4 * 32, smem, st>>>(prm);
   }
@@ -815,19 +873,21 @@ static int launch_fwd(TAParams& prm, cudaStream_t st) {
   return check_launch("temporal_attn_fwd");
 }
 
-template <int DH, int L>
+template <int DH, int L, bool RAGGED = false>
 static int launch_bwd(TAParams& prm, cudaStream_t st) {
   choose_geom(prm.D, L, prm.H, DH, 4, L == 8, is_fusable(prm, prm.H * DH), &prm.g, prm.B);
   const int smem = tile_smem(prm.g, 4);
   const int64_t grid = (int64_t)prm.B * (prm.D / prm.g.P) * (prm.H / prm.g.HG);
   const int n_items = ((prm.g.P + TACfg<DH, L>::PP - 1) / TACfg<DH, L>::PP) * prm.g.HG;
-  if (try_launch_cgeom<DH, L, true>(prm, (unsigned)grid, smem, n_items, st)) {
+  bool launched = false;
+  if constexpr (!RAGGED) launched = try_launch_cgeom<DH, L, true>(prm, (unsigned)grid, smem, n_items, st);
+  if (launched) {
   } else if (n_items >= 16) {
-    auto kern = temporal_attn_bwd_kernel<DH, L, 8>;
+    auto kern = temporal_attn_bwd_kernel<DH, L, 8, TileGeom, RAGGED>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     kern<<<(unsigned)grid, 8 * 32, smem, st>>>(prm);
   } else {
-    auto kern = temporal_attn_bwd_kernel<DH, L, 4>;
+    auto kern = temporal_attn_bwd_kernel<DH, L, 4, TileGeom, RAGGED>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     kern<<<(unsigned)grid, 4 * 32, smem, st>>>(prm);
   }
@@ -835,47 +895,91 @@ static int launch_bwd(TAParams& prm, cudaStream_t st) {
   return check_launch("temporal_attn_bwd");
 }
 
-#define MC_DISPATCH_DH(L_, FN)                              \
+#define MC_DISPATCH_DH(L_, FN, RG)                          \
   switch (DH) {                                             \
-    case 8: return FN<8, L_>(prm, st);                      \
-    case 16: return FN<16, L_>(prm, st);                    \
-    case 32: return FN<32, L_>(prm, st);                    \
-    case 40: return FN<40, L_>(prm, st);                    \
-    case 64: return FN<64, L_>(prm, st);                    \
-    case 80: return FN<80, L_>(prm, st);                    \
-    case 128: return FN<128, L_>(prm, st);                  \
-    case 160: return FN<160, L_>(prm, st);                  \
+    case 8: return FN<8, L_, RG>(prm, st);                  \
+    case 16: return FN<16, L_, RG>(prm, st);                \
+    case 32: return FN<32, L_, RG>(prm, st);                \
+    case 40: return FN<40, L_, RG>(prm, st);                \
+    case 64: return FN<64, L_, RG>(prm, st);                \
+    case 80: return FN<80, L_, RG>(prm, st);                \
+    case 128: return FN<128, L_, RG>(prm, st);              \
+    case 160: return FN<160, L_, RG>(prm, st);              \
     default: break;                                         \
   }
 
-#if MC_TA_PART != 2
+// Ragged launches (1 <= L <= 32, L not a tile length); they live in their own translation units (MC_TA_PART 3 / 4).
+// MC_E_UNSUPPORTED (error message left to the caller) for a head dim without an instantiation.
+int dispatch_fwd_ragged(TAParams& prm, int L, int DH, cudaStream_t st);
+int dispatch_bwd_ragged(TAParams& prm, int L, int DH, cudaStream_t st);
+
+#if MC_TA_PART == 0 || MC_TA_PART == 1
 static int dispatch_fwd(TAParams& prm, int L, int DH, cudaStream_t st) {
-  if (L == 8) { MC_DISPATCH_DH(8, launch_fwd) }
-  if (L == 16) { MC_DISPATCH_DH(16, launch_fwd) }
-  if (L == 32) { MC_DISPATCH_DH(32, launch_fwd) }
-  set_error("temporal_attn_fwd: unsupported L=%d / DH=%d (L in {8,16,32}; DH in {8,16,32,40,64,80,128,160})", L, DH);
+  if (L == 8) { MC_DISPATCH_DH(8, launch_fwd, false) }
+  if (L == 16) { MC_DISPATCH_DH(16, launch_fwd, false) }
+  if (L == 32) { MC_DISPATCH_DH(32, launch_fwd, false) }
+  if (L != 8 && L != 16 && L != 32) {
+    const int rc = dispatch_fwd_ragged(prm, L, DH, st);
+    if (rc != MC_E_UNSUPPORTED) return rc;
+  }
+  set_error("temporal_attn_fwd: unsupported L=%d / DH=%d (L in 1..32; DH in {8,16,32,40,64,80,128,160})", L, DH);
   return MC_E_UNSUPPORTED;
 }
 
 #endif
-#if MC_TA_PART != 1
+#if MC_TA_PART == 0 || MC_TA_PART == 2
 static int dispatch_bwd(TAParams& prm, int L, int DH, cudaStream_t st) {
-  if (L == 8) { MC_DISPATCH_DH(8, launch_bwd) }
-  if (L == 16) { MC_DISPATCH_DH(16, launch_bwd) }
-  if (L == 32) { MC_DISPATCH_DH(32, launch_bwd) }
-  set_error("temporal_attn_bwd: unsupported L=%d / DH=%d (L in {8,16,32}; DH in {8,16,32,40,64,80,128,160})", L, DH);
+  if (L == 8) { MC_DISPATCH_DH(8, launch_bwd, false) }
+  if (L == 16) { MC_DISPATCH_DH(16, launch_bwd, false) }
+  if (L == 32) { MC_DISPATCH_DH(32, launch_bwd, false) }
+  if (L != 8 && L != 16 && L != 32) {
+    const int rc = dispatch_bwd_ragged(prm, L, DH, st);
+    if (rc != MC_E_UNSUPPORTED) return rc;
+  }
+  set_error("temporal_attn_bwd: unsupported L=%d / DH=%d (L in 1..32; DH in {8,16,32,40,64,80,128,160})", L, DH);
+  return MC_E_UNSUPPORTED;
+}
+
+#endif
+#if MC_TA_PART == 0 || MC_TA_PART >= 3
+// tile length a clip of L frames runs in
+static int tile_len(int L) { return L <= 8 ? 8 : (L <= 16 ? 16 : 32); }
+
+#endif
+#if MC_TA_PART == 0 || MC_TA_PART == 3
+int dispatch_fwd_ragged(TAParams& prm, int L, int DH, cudaStream_t st) {
+  switch (tile_len(L)) {
+    case 8: { MC_DISPATCH_DH(8, launch_fwd, true) } break;
+    case 16: { MC_DISPATCH_DH(16, launch_fwd, true) } break;
+    default: { MC_DISPATCH_DH(32, launch_fwd, true) } break;
+  }
+  return MC_E_UNSUPPORTED;
+}
+
+#endif
+#if MC_TA_PART == 0 || MC_TA_PART == 4
+int dispatch_bwd_ragged(TAParams& prm, int L, int DH, cudaStream_t st) {
+  switch (tile_len(L)) {
+    case 8: { MC_DISPATCH_DH(8, launch_bwd, true) } break;
+    case 16: { MC_DISPATCH_DH(16, launch_bwd, true) } break;
+    default: { MC_DISPATCH_DH(32, launch_bwd, true) } break;
+  }
   return MC_E_UNSUPPORTED;
 }
 
 #endif
 }  // namespace mc
 
-#if MC_TA_PART != 2
+#if MC_TA_PART == 0 || MC_TA_PART == 1
 extern "C" int mc_temporal_attn_fwd(const void* q, const void* k, const void* v, mc_temporal_layout qkv_layout,
                                     void* o, mc_temporal_layout o_layout, void* probs, void* top_val,
                                     uint8_t* top_idx, const uint8_t* gather_idx, void* gathered, int B, int D, int L,
                                     int H, int DH, float scale, void* stream) {
   using namespace mc;
+  if (L < 1 || L > 32) {  // the motion module's positional encoding has 32 entries (max_len)
+    set_error("temporal_attn_fwd: L=%d frames outside the supported range 1..32", L);
+    return MC_E_UNSUPPORTED;
+  }
   if (!q || !k || (o && !v) || B <= 0 || D <= 0 || H <= 0) {
     set_error("temporal_attn_fwd: null q/k (or o without v) or non-positive dims");
     return MC_E_INVALID;
@@ -904,17 +1008,22 @@ extern "C" int mc_temporal_attn_fwd(const void* q, const void* k, const void* v,
   prm.D = D;
   prm.H = H;
   prm.scale = scale;
+  prm.L = L;
   return dispatch_fwd(prm, L, DH, (cudaStream_t)stream);
 }
 
 #endif
-#if MC_TA_PART != 1
+#if MC_TA_PART == 0 || MC_TA_PART == 2
 extern "C" int mc_temporal_attn_bwd(const void* q, const void* k, const void* v, mc_temporal_layout qkv_layout,
                                     const void* d_o, mc_temporal_layout do_layout, const void* d_probs,
                                     const uint8_t* gather_idx, const void* d_gathered, void* dq, void* dk, void* dv,
                                     mc_temporal_layout g_layout, int B, int D, int L, int H, int DH, float scale,
                                     void* stream) {
   using namespace mc;
+  if (L < 1 || L > 32) {  // the motion module's positional encoding has 32 entries (max_len)
+    set_error("temporal_attn_bwd: L=%d frames outside the supported range 1..32", L);
+    return MC_E_UNSUPPORTED;
+  }
   if (!q || !k || !dq || !dk || (d_o && !v) || B <= 0 || D <= 0 || H <= 0) {
     set_error("temporal_attn_bwd: null q/k/dq/dk (or d_o without v) or non-positive dims");
     return MC_E_INVALID;
@@ -945,6 +1054,7 @@ extern "C" int mc_temporal_attn_bwd(const void* q, const void* k, const void* v,
   prm.D = D;
   prm.H = H;
   prm.scale = scale;
+  prm.L = L;
   return dispatch_bwd(prm, L, DH, (cudaStream_t)stream);
 }
 #endif

@@ -226,8 +226,8 @@ class CrossAttention(nn.Module):
         if attention_mask is not None:
             raise NotImplementedError
         bh, s, dh = query.shape
-        if s not in (8, 16, 32) or key.shape[1] != s:
-            raise NotImplementedError("get_attention_scores: temporal shapes only (S = key length in {8, 16, 32}); "
+        if not 1 <= s <= 32 or key.shape[1] != s:
+            raise NotImplementedError("get_attention_scores: temporal shapes only (S = key length in 1..32); "
                                       "spatial probabilities are never materialised on this path")
         h = self.heads
         to_bfpc = lambda t: t.reshape(bh // h, h, s, dh).permute(0, 2, 1, 3).reshape(1, bh // h, s, h * dh) \

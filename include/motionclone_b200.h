@@ -204,6 +204,18 @@ int mc_groupnorm_nhwc_stats(const void* workspace, void* stats, int N, int HW, i
 int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz, void* dx,
                           const void* stats, const void* gamma, const void* beta, void* workspace,
                           int64_t workspace_bytes, int N, int HW, int C, int G, int fuse_silu, void* stream);
+/* Batch-invariant forms of the two calls above: x holds `samples` samples of N / samples frames each (N % samples == 0,
+ * any frame order). The per-frame split of the reduction is chosen from the frames of ONE sample, so each frame's
+ * statistics and gradient sums are added in the same order as in a call on its own sample alone: every sample gets the
+ * bits of its single-sample call. mc_groupnorm_nhwc / mc_groupnorm_nhwc_bwd are these with samples = 1 (the split is
+ * then chosen from all N frames). Same workspace size and zero-ticket rule; N <= 1024 frames in total. */
+int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, int frames_per_bias_row, void* y, const void* gamma,
+                              const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW, int C, int G,
+                              int samples, float eps, int fuse_silu, void* stream);
+int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz, void* dx,
+                                  const void* stats, const void* gamma, const void* beta, void* workspace,
+                                  int64_t workspace_bytes, int N, int HW, int C, int G, int samples, int fuse_silu,
+                                  void* stream);
 int mc_layernorm_bwd(const void* x, const void* dy, void* dx, const void* gamma, const void* pre_bias, int64_t rows, int C,
                      float eps, void* stream);
 int mc_geglu_bwd(const void* in, const void* dout, void* din, int64_t T, int I, void* stream);

@@ -531,15 +531,18 @@ struct GnTiling {
 };
 
 // `tensors` tiles of <= tile_bytes each per stage, two stages (64 KB per CTA -> 3 CTAs per SM; the backward kernels hold
-// more registers: 2). ONE wave: at most 132 x ctas_per_sm CTAs in the grid, each walking ceil(tiles / S) tiles through its two-stage pipeline (a grid of 1.5 waves costs
-// two: measured on the 16 x 64 x 64 x 320 layers).
-static GnTiling gn_tiling(int N, int HW, int C, int NT, int tensors, int tile_bytes, int ctas_per_sm) {
+// more registers: 2). ONE wave per sample: at most 132 x ctas_per_sm CTAs for the `frames_per_sample` frames of one
+// sample, each walking ceil(tiles / S) tiles through its two-stage pipeline (a grid of 1.5 waves costs two: measured on
+// the 16 x 64 x 64 x 320 layers).
+// S and PX depend on the frames of ONE sample, never on how many samples share the launch: a frame's fp32 statistics
+// are summed in an order fixed by (S, PX), so a batched call gives every sample the bits of its own single-sample call.
+static GnTiling gn_tiling(int frames_per_sample, int HW, int C, int NT, int tensors, int tile_bytes, int ctas_per_sm) {
   GnTiling t;
   t.PX = tile_bytes / (C * 2);
   if (t.PX < 1) t.PX = 1;
   if (t.PX > HW) t.PX = HW;
   const int tiles = (HW + t.PX - 1) / t.PX;
-  t.S = (132 * ctas_per_sm) / N;
+  t.S = (132 * ctas_per_sm) / frames_per_sample;
   if (t.S < 1) t.S = 1;
   if (t.S > tiles) t.S = tiles;
   if (t.S > kGnMaxSplits) t.S = kGnMaxSplits;
@@ -555,9 +558,13 @@ static void gn_allow_smem(K kern, int smem) {
   if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
-static int gn_check(const char* what, int N, int HW, int C, int G) {
+static int gn_check(const char* what, int N, int HW, int C, int G, int samples) {
   if (N <= 0 || HW <= 0) {
     set_error("%s: non-positive dims", what);
+    return MC_E_INVALID;
+  }
+  if (samples <= 0 || N % samples != 0) {
+    set_error("%s: samples must be positive and divide N (got N=%d samples=%d)", what, N, samples);
     return MC_E_INVALID;
   }
   if (C % 8 != 0 || C % G != 0 || C > 4096 || G > 128 || N > kGnTicketBytes / 4) {
@@ -587,15 +594,15 @@ extern "C" int64_t mc_groupnorm_workspace_bytes(int N, int G) {
   return mc::kGnTicketBytes + (int64_t)N * G * 2 * sizeof(float) + (int64_t)N * mc::kGnMaxSplits * G * 3 * sizeof(float);
 }
 
-extern "C" int mc_groupnorm_nhwc(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
-                                 const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes, int N,
-                                 int HW, int C, int G, float eps, int fuse_silu, void* stream) {
+extern "C" int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
+                                         const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes,
+                                         int N, int HW, int C, int G, int samples, float eps, int fuse_silu, void* stream) {
   using namespace mc;
   if (!x || !y || !gamma || !beta || !workspace) {
     set_error("groupnorm_nhwc: null pointer");
     return MC_E_INVALID;
   }
-  int rc = gn_check("groupnorm_nhwc", N, HW, C, G);
+  int rc = gn_check("groupnorm_nhwc", N, HW, C, G, samples);
   if (rc != MC_OK) return rc;
   if (chan_bias != nullptr && frames_per_bias_row <= 0) {
     set_error("groupnorm_nhwc: frames_per_bias_row must be positive when chan_bias is given");
@@ -609,7 +616,7 @@ extern "C" int mc_groupnorm_nhwc(const void* x, const void* chan_bias, int frame
   const GnLaunch L = gn_launch(C);
   const GnWorkspace w = gn_workspace(workspace, N, G);
   cudaStream_t st = (cudaStream_t)stream;
-  const GnTiling T = gn_tiling(N, HW, C, L.NT, 1, kGnTileBytes, 3);
+  const GnTiling T = gn_tiling(N / samples, HW, C, L.NT, 1, kGnTileBytes, 3);
   gn_allow_smem(groupnorm_stats_kernel, T.smem);
   groupnorm_stats_kernel<<<dim3(N, T.S), L.NT, T.smem, st>>>((const __half*)x, (const __half*)chan_bias,
                                                              frames_per_bias_row, w.partial, w.finalised, w.tickets, HW, C,
@@ -632,6 +639,13 @@ extern "C" int mc_groupnorm_nhwc(const void* x, const void* chan_bias, int frame
   return check_launch("groupnorm_apply");
 }
 
+extern "C" int mc_groupnorm_nhwc(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
+                                 const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes, int N,
+                                 int HW, int C, int G, float eps, int fuse_silu, void* stream) {
+  return mc_groupnorm_nhwc_batched(x, chan_bias, frames_per_bias_row, y, gamma, beta, workspace, workspace_bytes, N, HW,
+                                   C, G, 1, eps, fuse_silu, stream);
+}
+
 extern "C" int mc_groupnorm_nhwc_stats(const void* workspace, void* stats, int N, int HW, int G, float eps, void* stream) {
   using namespace mc;
   (void)HW, (void)eps;  // kept in the signature: the statistics are final once mc_groupnorm_nhwc has run
@@ -649,15 +663,16 @@ extern "C" int mc_groupnorm_nhwc_stats(const void* workspace, void* stats, int N
   return MC_OK;
 }
 
-extern "C" int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz,
-                                     void* dx, const void* stats, const void* gamma, const void* beta, void* workspace,
-                                     int64_t workspace_bytes, int N, int HW, int C, int G, int fuse_silu, void* stream) {
+extern "C" int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bias, int frames_per_bias_row,
+                                             const void* dz, void* dx, const void* stats, const void* gamma,
+                                             const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW,
+                                             int C, int G, int samples, int fuse_silu, void* stream) {
   using namespace mc;
   if (!x || !dz || !dx || !stats || !gamma || !beta || !workspace) {
     set_error("groupnorm_nhwc_bwd: null pointer");
     return MC_E_INVALID;
   }
-  int rc = gn_check("groupnorm_nhwc_bwd", N, HW, C, G);
+  int rc = gn_check("groupnorm_nhwc_bwd", N, HW, C, G, samples);
   if (rc != MC_OK) return rc;
   if (chan_bias != nullptr && frames_per_bias_row <= 0) {
     set_error("groupnorm_nhwc_bwd: frames_per_bias_row must be positive when chan_bias is given");
@@ -670,7 +685,7 @@ extern "C" int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int f
   const GnLaunch L = gn_launch(C);
   const GnWorkspace w = gn_workspace(workspace, N, G);
   cudaStream_t st = (cudaStream_t)stream;
-  const GnTiling T = gn_tiling(N, HW, C, L.NT, 2, kGnTileBytes / 2, 2);
+  const GnTiling T = gn_tiling(N / samples, HW, C, L.NT, 2, kGnTileBytes / 2, 2);
   const __half *xp = (const __half*)x, *cbp = (const __half*)chan_bias, *dzp = (const __half*)dz;
   const __half *gp = (const __half*)gamma, *bp = (const __half*)beta;
   if (fuse_silu) {
@@ -702,4 +717,11 @@ extern "C" int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int f
   }
   count_launch();
   return check_launch("groupnorm_bwd_apply");
+}
+
+extern "C" int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz,
+                                     void* dx, const void* stats, const void* gamma, const void* beta, void* workspace,
+                                     int64_t workspace_bytes, int N, int HW, int C, int G, int fuse_silu, void* stream) {
+  return mc_groupnorm_nhwc_bwd_batched(x, chan_bias, frames_per_bias_row, dz, dx, stats, gamma, beta, workspace,
+                                       workspace_bytes, N, HW, C, G, 1, fuse_silu, stream);
 }

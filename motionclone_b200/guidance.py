@@ -161,22 +161,55 @@ def obtain_motion_representation(self, generator=None, motion_representation_pat
 # ----------------------------------------------------------------------------------------------------------------
 # 3. compute_temp_loss / 6. get_temp_attn_prob
 # ----------------------------------------------------------------------------------------------------------------
+def _check_representation(rep, frames: int, label: str = "motion representation"):
+    """Value / index tensors of shape [N, heads, frames, 1] with every index < frames (a stale or foreign .pt must fail
+    here, as torch.gather would at :91-92)."""
+    for k, (val, idx) in rep.items():
+        if val.shape != idx.shape or val.dim() != 4 or val.shape[-1] != 1:
+            raise ValueError(f"{label} '{k}': expected value / index tensors of shape [N, heads, L, 1], "
+                             f"got {tuple(val.shape)} / {tuple(idx.shape)}")
+        if val.shape[-2] != frames:
+            raise ValueError(f"{label} '{k}': {val.shape[-2]} frames, the video has {frames}")
+        if int(idx.max()) >= frames:
+            raise ValueError(f"{label} '{k}': index {int(idx.max())} >= video_length {frames}")
+
+
+def _rep_to_device(rep, device):
+    out = {k: (v[0].to(device=device, dtype=torch.float16).contiguous(),
+               v[1].to(device=device, dtype=torch.uint8).contiguous()) for k, v in rep.items()}
+    for k, (val, _) in out.items():
+        _check_representation({k: out[k]}, val.shape[-2])
+    return out
+
+
 def _device_representation(self, device):
     cache = getattr(self, "_repr_on_device", None)
     if cache is None or cache[0] is not self.motion_representation_dict or cache[1] != device:
-        rep = {k: (v[0].to(device=device, dtype=torch.float16).contiguous(),
-                   v[1].to(device=device, dtype=torch.uint8).contiguous())
-               for k, v in self.motion_representation_dict.items()}
-        for k, (val, idx) in rep.items():  # a stale / foreign .pt must fail here, as torch.gather would (:91-92)
-            frames = val.shape[-2]
-            if val.shape != idx.shape or val.dim() != 4 or val.shape[-1] != 1:
-                raise ValueError(f"motion representation '{k}': expected value / index tensors of shape [N, heads, L, 1], "
-                                 f"got {tuple(val.shape)} / {tuple(idx.shape)}")
-            if int(idx.max()) >= frames:
-                raise ValueError(f"motion representation '{k}': index {int(idx.max())} >= video_length {frames}")
-        self._repr_on_device = (self.motion_representation_dict, device, rep)
+        self._repr_on_device = (self.motion_representation_dict, device,
+                                _rep_to_device(self.motion_representation_dict, device))
         cache = self._repr_on_device
     return cache[2]
+
+
+def _device_batch(self, device, batch: int):
+    """Per-sample device copies of the B representations the sampling loop runs with (`_sample_reps`, one dict per
+    sample; a shared dict is copied once) and, per guided module, the B index tensors concatenated to [B*d, heads, f, 1]:
+    the row order ((b*d + p)*heads + h)*f + frame in which the temporal kernel reads its `gather_idx`. Made once per
+    sample_video call, not once per step."""
+    reps = getattr(self, "_sample_reps", None) or [self.motion_representation_dict] * batch
+    cache = getattr(self, "_batch_on_device", None)
+    if (cache is None or cache[1] != device or len(cache[0]) != len(reps)
+            or any(a is not b for a, b in zip(cache[0], reps))):
+        per_dict = {}
+        for r in reps:
+            if id(r) not in per_dict:
+                per_dict[id(r)] = _device_representation(self, device) if r is self.motion_representation_dict \
+                    else _rep_to_device(r, device)
+        dev_reps = [per_dict[id(r)] for r in reps]
+        cat_idx = {k: (dev_reps[0][k][1] if len(reps) == 1 else torch.cat([d[k][1] for d in dev_reps]))
+                   for k in dev_reps[0]}
+        self._batch_on_device = cache = (list(reps), device, dev_reps, cat_idx)
+    return cache[2], cache[3]
 
 
 def compute_temp_loss(self, temp_attn_prob_control_dict):
@@ -215,11 +248,87 @@ def get_temp_attn_prob(self, index_select=None):
 # ----------------------------------------------------------------------------------------------------------------
 # 4. sample_video / 5. single_step_video
 # ----------------------------------------------------------------------------------------------------------------
+def _load_representation(rep):
+    return torch.load(rep) if isinstance(rep, str) else rep  # :154 (same on-disk format as :81)
+
+
+def _batch_size(self, text_embeddings, noisy_latents, generator, motion_representation) -> int:
+    """B of a sample_video call, from every input that carries it; any disagreement is a ValueError."""
+    if text_embeddings.dim() != 3 or text_embeddings.shape[0] < 2 or text_embeddings.shape[0] % 2:
+        raise ValueError(f"prompt embeddings must be [2B, 77, c] = [uncond_1..B, cond_1..B], got "
+                         f"{tuple(text_embeddings.shape)}")
+    counts = {"prompt embeddings (2B rows)": text_embeddings.shape[0] // 2}
+    if noisy_latents is not None:
+        if noisy_latents.dim() != 5:
+            raise ValueError(f"noisy_latents must be [B, 4, f, h/8, w/8], got {tuple(noisy_latents.shape)}")
+        counts["noisy_latents"] = noisy_latents.shape[0]
+    if isinstance(generator, (list, tuple)):
+        counts["generators"] = len(generator)
+    if isinstance(motion_representation, (list, tuple)):
+        counts["motion representations"] = len(motion_representation)
+    if len(set(counts.values())) != 1:
+        raise ValueError("batch size mismatch: " + ", ".join(f"{k} {v}" for k, v in counts.items()))
+    return next(iter(counts.values()))
+
+
+def _resolve_representations(self, motion_representation, batch: int, frames: int):
+    """The B representation dicts of a call, checked on the host before anything runs on the device. None: the pipeline's
+    own (obtain_motion_representation, motion_representation_path or motion_representation_dict), shared by all samples;
+    one dict / path: shared; a list of B dicts / paths: one per sample."""
+    if motion_representation is None:
+        path = getattr(self, "motion_representation_path", None)
+        if path is not None and getattr(self, "_repr_source", None) != path:
+            self.motion_representation_dict = torch.load(path)  # :154
+            self._repr_source = path
+        elif getattr(self, "motion_representation_dict", None) is None:
+            raise ValueError("no motion representation: run obtain_motion_representation, set "
+                             "motion_representation_path or pass motion_representation")
+        reps = [self.motion_representation_dict] * batch
+    elif isinstance(motion_representation, (list, tuple)):
+        reps = [_load_representation(r) for r in motion_representation]
+    else:
+        self.motion_representation_dict = _load_representation(motion_representation)
+        self.motion_representation_path = self._repr_source = None
+        reps = [self.motion_representation_dict] * batch
+    names = list(guided_modules(self))
+    prev = getattr(self, "_reps_checked", None)  # the same dicts as the last call: checked then (no device reads per call)
+    if prev is not None and prev[1] == frames and len(prev[0]) == len(reps) and all(a is b for a, b in zip(prev[0], reps)):
+        return reps
+    checked = set()
+    for i, rep in enumerate(reps):
+        if id(rep) in checked:
+            continue
+        missing = [n for n in names if n not in rep]
+        if missing:
+            raise ValueError(f"motion representation {i}: no entry for guided module(s) {missing}")
+        _check_representation({n: rep[n] for n in names}, frames, f"motion representation {i}")
+        checked.add(id(rep))
+    self._reps_checked = (list(reps), frames)
+    return reps
+
+
 def sample_video(self, eta: float = 0.0, generator=None, noisy_latents: Optional[torch.Tensor] = None,
-                 add_controlnet: bool = False, return_latents: bool = False):
-    """:102-171. `return_latents=True` skips the VAE decode (off the measured path, SURVEY.md §8d) and returns the
-    final latents `[1, 4, f, h/8, w/8]`."""
+                 add_controlnet: bool = False, return_latents: bool = False, motion_representation=None):
+    """:102-171, for a batch of B samples sharing f, h, w, the schedule and the guidance settings. B comes from the
+    inputs: `noisy_latents` [B, 4, f, h/8, w/8] or a list of B generators, prompt embeddings [2B, 77, c] in the order
+    [uncond_1..B, cond_1..B], and `motion_representation`: None (the pipeline's own), one dict or path shared by all
+    samples, or a list of B dicts or paths. Sample s gets what a B = 1 call on sample s alone gets, up to the
+    batch-size-dependent algorithms of cuBLAS / cuDNN (DESIGN.md §5). `return_latents=True` skips the VAE decode (off
+    the measured path, SURVEY.md §8d) and returns the final latents [B, 4, f, h/8, w/8]. After a call, `last_loss` is
+    the summed guidance loss of the last guided step and `last_loss_per_sample` [B] its per-sample terms."""
     cfg = self.input_config
+    device = self._execution_device
+    text_embeddings = self._encode_prompt(_cfg_get(cfg, "new_prompt"), device, 1, True,
+                                          _cfg_get(cfg, "negative_prompt"))
+    batch_size = _batch_size(self, text_embeddings, noisy_latents, generator, motion_representation)
+    frames = _cfg_get(cfg, "video_length")
+    if add_controlnet and batch_size > 1:
+        raise NotImplementedError(f"SparseCtrl (add_controlnet=True) runs one sample per call; got a batch of "
+                                  f"{batch_size}: call sample_video once per sample")
+    if 2 * batch_size * frames > 1024:  # the plain step's b = 2B UNet pass: GroupNorm takes at most 1024 frames
+        raise ValueError(f"a batch of {batch_size} x {frames} frames exceeds 1024 frames in the b = 2B UNet pass: "
+                         f"use at most {1024 // (2 * frames)} samples per call")
+    reps = _resolve_representations(self, motion_representation, batch_size, frames)
     self.add_controlnet = add_controlnet
     if add_controlnet:  # :111-128 — image files + VAE encode are off the path: the caller passes their result
         images = _cfg_get(cfg, "controlnet_images")
@@ -228,25 +337,20 @@ def sample_video(self, eta: float = 0.0, generator=None, noisy_latents: Optional
                                       "input_config.controlnet_images [1, c, n_images, h, w] (latents x 0.18215 for the "
                                       "simplified embedding, RGB in [0, 1] otherwise)")
         self.controlnet_images = images.to(device=self.device, dtype=self.unet.dtype)
-    batch_size = 1
-    device = self._execution_device
-    self.text_embeddings = self._encode_prompt(_cfg_get(cfg, "new_prompt"), device, 1, True,
-                                               _cfg_get(cfg, "negative_prompt"))
-    noisy_latents = self.prepare_latents(batch_size, self.unet.config.in_channels, _cfg_get(cfg, "video_length"),
+    self.text_embeddings = text_embeddings
+    noisy_latents = self.prepare_latents(batch_size, self.unet.config.in_channels, frames,
                                          _cfg_get(cfg, "height"), _cfg_get(cfg, "width"), self.text_embeddings.dtype,
                                          device, generator, noisy_latents)
-    path = getattr(self, "motion_representation_path", None)
-    if path is not None and getattr(self, "_repr_source", None) != path:
-        self.motion_representation_dict = torch.load(path)  # :154
-        self._repr_source = path
-    elif getattr(self, "motion_representation_dict", None) is None:
-        raise ValueError("no motion representation: run obtain_motion_representation or set motion_representation_path")
     self.motion_scale = _cfg_get(cfg, "motion_guidance_weight")
     extra_step_kwargs = self.prepare_extra_step_kwargs(generator, eta)
-    with self.progress_bar(total=_cfg_get(cfg, "inference_steps")) as bar:
-        for step_index, step_t in enumerate(self.scheduler.timesteps_host):
-            noisy_latents = self.single_step_video(noisy_latents, step_index, int(step_t), extra_step_kwargs)
-            bar.update()
+    self._sample_reps = reps
+    try:
+        with self.progress_bar(total=_cfg_get(cfg, "inference_steps")) as bar:
+            for step_index, step_t in enumerate(self.scheduler.timesteps_host):
+                noisy_latents = self.single_step_video(noisy_latents, step_index, int(step_t), extra_step_kwargs)
+                bar.update()
+    finally:  # a direct single_step_video call guides with motion_representation_dict
+        self._sample_reps = None
     if return_latents:
         return noisy_latents
     return self.decode_latents(noisy_latents)
@@ -287,23 +391,38 @@ class _GraphedUNetForward:
         return self.out
 
 
-def _unet_nograd(self, sample, step_t, text, step_index):
-    """No-grad UNet forward without SparseCtrl residuals: replayed from a CUDA graph when the pipeline allows it (the
-    timestep then comes from the scheduler's DEVICE copy of the schedule: no host value is baked into the graph)."""
-    if not getattr(self, "use_cuda_graphs", False) or not sample.is_cuda:
-        return self.unet(sample, step_t, encoder_hidden_states=text).sample
-    step_t = self.scheduler.timesteps[step_index]  # 0-dim int64 device tensor, no sync
-    graphs = self.__dict__.setdefault("_unet_graphs", {})
-    key = (tuple(sample.shape), sample.dtype, tuple(text.shape))
-    g = graphs.get(key)
-    if g is None:
-        g = graphs[key] = _GraphedUNetForward(self.unet, sample, step_t, text)
-    return g(sample, step_t, text)
+def _unet_nograd(self, sample, step_t, text, step_index, samples: int = 1):
+    """No-grad UNet forward of `samples` samples without SparseCtrl residuals: replayed from a CUDA graph when the
+    pipeline allows it (the timestep then comes from the scheduler's DEVICE copy of the schedule: no host value is baked
+    into the graph). The GroupNorm tiling depends on `samples`, so it is part of the graph key."""
+    with ops.batch_samples(samples):
+        if not getattr(self, "use_cuda_graphs", False) or not sample.is_cuda:
+            return self.unet(sample, step_t, encoder_hidden_states=text).sample
+        step_t = self.scheduler.timesteps[step_index]  # 0-dim int64 device tensor, no sync
+        graphs = self.__dict__.setdefault("_unet_graphs", {})
+        key = (tuple(sample.shape), sample.dtype, tuple(text.shape), samples)
+        g = graphs.get(key)
+        if g is None:
+            g = graphs[key] = _GraphedUNetForward(self.unet, sample, step_t, text)
+        return g(sample, step_t, text)
+
+
+def _step_weight(self, step_index, loss):
+    """Warm-up / cool-down ramp of the guidance loss (:228-234; the cool-down test is a strict '>')."""
+    cfg = self.input_config
+    guidance_steps = _cfg_get(cfg, "guidance_steps")
+    if step_index < _cfg_get(cfg, "warm_up_steps"):
+        loss = ((step_index + 1) / _cfg_get(cfg, "warm_up_steps")) * loss
+    if step_index > guidance_steps - _cfg_get(cfg, "cool_up_steps"):
+        loss = ((guidance_steps - step_index) / _cfg_get(cfg, "cool_up_steps")) * loss
+    return loss
 
 
 def single_step_video(self, noisy_latents, step_index, step_t, extra_step_kwargs):
-    """:173-257."""
+    """:173-257 for a batch of B = noisy_latents.shape[0] samples (text embeddings [uncond_1..B, cond_1..B])."""
     cfg = self.input_config
+    B = noisy_latents.shape[0]
+    text_u, text_c = self.text_embeddings[:B], self.text_embeddings[B:]
     down = mid = None
     if getattr(self, "add_controlnet", False):  # :176-197: SparseCtrl at b=2 ([uncond, cond]) under no_grad
         down, mid = _controlnet_residuals(self, noisy_latents.expand(2, -1, -1, -1, -1), step_t, self.text_embeddings,
@@ -311,30 +430,39 @@ def single_step_video(self, noisy_latents, step_index, step_t, extra_step_kwargs
     guidance_steps = _cfg_get(cfg, "guidance_steps")
     cfg_scale = _cfg_get(cfg, "cfg_scale")
     if step_index < guidance_steps:
-        rep = _device_representation(self, noisy_latents.device)
+        dev_reps, cat_idx = _device_batch(self, noisy_latents.device, B)
         control_latents = noisy_latents.clone().detach()
         control_latents.requires_grad = True
         with torch.no_grad():
             _set_processor_mode(self, None)
             if down is None:
-                eps_u = _unet_nograd(self, noisy_latents, step_t, self.text_embeddings[[0]], step_index)
+                eps_u = _unet_nograd(self, noisy_latents, step_t, text_u, step_index, samples=B)
             else:
-                eps_u = self.unet(noisy_latents, step_t, encoder_hidden_states=self.text_embeddings[[0]],
+                eps_u = self.unet(noisy_latents, step_t, encoder_hidden_states=text_u,
                                   down_block_additional_residuals=[r[0:1] for r in down],
                                   mid_block_additional_residual=mid[0:1]).sample
-        _set_processor_mode(self, "gather", {k: v[1] for k, v in rep.items()})
-        eps_c = self.unet(control_latents, step_t, encoder_hidden_states=self.text_embeddings[[1]],
-                          down_block_additional_residuals=None if down is None else [r[1:2] for r in down],
-                          mid_block_additional_residual=None if mid is None else mid[1:2]).sample
+        _set_processor_mode(self, "gather", cat_idx)
+        with ops.batch_samples(B):
+            eps_c = self.unet(control_latents, step_t, encoder_hidden_states=text_c,
+                              down_block_additional_residuals=None if down is None else [r[1:2] for r in down],
+                              mid_block_additional_residual=None if mid is None else mid[1:2]).sample
         gathered = {name: m.processor.gathered for name, m in guided_modules(self).items()}
-        loss_motion = self.motion_scale * self.compute_temp_loss(gathered)
-        if step_index < _cfg_get(cfg, "warm_up_steps"):  # :228-230
-            loss_motion = ((step_index + 1) / _cfg_get(cfg, "warm_up_steps")) * loss_motion
-        if step_index > guidance_steps - _cfg_get(cfg, "cool_up_steps"):  # :232-234 (strict '>')
-            loss_motion = ((guidance_steps - step_index) / _cfg_get(cfg, "cool_up_steps")) * loss_motion
+        # one loss launch per sample on its own contiguous rows: each sample's value and gradient are those of B = 1
+        losses = []
+        for s in range(B):
+            cur, ref = [], []
+            for name, p in gathered.items():
+                d = p.shape[0] // B
+                cur.append(p[s * d:(s + 1) * d])
+                ref.append(dev_reps[s][name][0])
+            losses.append(_step_weight(self, step_index, self.motion_scale * ops.motion_loss(cur, ref)))
+        loss_motion = losses[0]
+        for extra in losses[1:]:
+            loss_motion = loss_motion + extra
         gradient = torch.autograd.grad(loss_motion, control_latents, allow_unused=True)[0]
         assert gradient is not None, f"Step {step_index}: grad is None"
         self.last_loss, self.last_gradient = loss_motion.detach(), gradient.detach()
+        self.last_loss_per_sample = torch.stack([l.detach() for l in losses])
         _set_processor_mode(self, None)
         out = self.scheduler.customized_step_fused(eps_c.detach(), eps_u, cfg_scale, step_index,
                                                    control_latents.detach(), score=gradient.detach(),
@@ -342,12 +470,13 @@ def single_step_video(self, noisy_latents, step_index, step_t, extra_step_kwargs
         return out.detach()
     with torch.no_grad():
         _set_processor_mode(self, None)
-        if down is None:
-            pair = _unet_nograd(self, noisy_latents.expand(2, -1, -1, -1, -1), step_t, self.text_embeddings, step_index)
+        if down is None:  # one b = 2B pass [x_1..B, x_1..B]; each CFG pair counts as one GroupNorm sample
+            pair = _unet_nograd(self, noisy_latents.repeat(2, 1, 1, 1, 1), step_t, self.text_embeddings, step_index,
+                                samples=B)
         else:
             pair = self.unet(noisy_latents.expand(2, -1, -1, -1, -1), step_t, encoder_hidden_states=self.text_embeddings,
                              down_block_additional_residuals=down, mid_block_additional_residual=mid).sample
-        out = self.scheduler.customized_step_fused(pair[[1]], pair[[0]], cfg_scale, step_index, noisy_latents,
+        out = self.scheduler.customized_step_fused(pair[B:], pair[:B], cfg_scale, step_index, noisy_latents,
                                                    score=None, **extra_step_kwargs)
     return out.detach()
 

@@ -4,6 +4,7 @@ else raises; there is no eager fallback."""
 from __future__ import annotations
 
 import ctypes
+from contextlib import contextmanager
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -316,6 +317,22 @@ def add_noise(x0: Tensor, noise: Tensor, alpha_t: Tensor) -> Tensor:
 # NHWC GroupNorm(+SiLU), LayerNorm, GEGLU (inference passes)
 # ----------------------------------------------------------------------------------------------------------------
 _gn_workspace = {}
+_gn_samples = 1
+
+
+@contextmanager
+def batch_samples(samples: int):
+    """GroupNorm calls made inside see their batch as `samples` samples of equal size (N = samples x frames per sample):
+    the kernels then split each frame's reduction as a call on one sample would, so every sample of a batched UNet pass
+    gets the GroupNorm bits of its own single-sample pass (include/motionclone_b200.h, mc_groupnorm_nhwc_batched)."""
+    global _gn_samples
+    if int(samples) < 1:
+        raise ValueError(f"batch_samples: need at least one sample, got {samples}")
+    prev, _gn_samples = _gn_samples, int(samples)
+    try:
+        yield
+    finally:
+        _gn_samples = prev
 
 
 def glue_kernels_ok(x: Tensor) -> bool:
@@ -354,21 +371,23 @@ def _check_chan_bias(x: Tensor, chan_bias: Optional[Tensor]):
 
 
 def groupnorm_nhwc(x: Tensor, weight: Tensor, bias: Tensor, groups: int, eps: float, silu: bool = False,
-                   chan_bias: Optional[Tensor] = None, want_stats: bool = False):
+                   chan_bias: Optional[Tensor] = None, want_stats: bool = False, samples: Optional[int] = None):
     """x: [N, C, h, w] in channels_last (physically [N, h, w, C]); returns the same format. `chan_bias` [NB, C]
     (N % NB == 0) is added to x first, row n // (N // NB) — the resnet's time-embedding add folded in.
-    `want_stats` also returns (mean, rstd) [N, groups, 2] fp32 for the backward."""
+    `want_stats` also returns (mean, rstd) [N, groups, 2] fp32 for the backward. `samples` (N % samples == 0; default:
+    the enclosing `batch_samples`, else 1) makes the result of each sample independent of the others in the batch."""
     _require(x, "x")
     if x.dim() != 4 or not x.is_contiguous(memory_format=torch.channels_last):
         raise ValueError("groupnorm_nhwc expects a 4-D channels_last tensor")
     chan_bias, fpr = _check_chan_bias(x, chan_bias)
     N, C, H, W = x.shape
+    samples = _gn_samples if samples is None else int(samples)
     weight, bias = _require_param(weight, "groupnorm weight", x, C), _require_param(bias, "groupnorm bias", x, C)
     y = torch.empty_like(x)  # preserves channels_last
     ws = _workspace(x, int(_lib.lib().mc_groupnorm_workspace_bytes(N, groups)))
-    st = _lib.lib().mc_groupnorm_nhwc(_ptr(x), _ptr(chan_bias), fpr, _ptr(y), _ptr(weight), _ptr(bias), _ptr(ws),
-                                      ws.numel(), N, H * W, C, groups, float(eps), int(silu), _stream())
-    _lib.check(st, "mc_groupnorm_nhwc")
+    st = _lib.lib().mc_groupnorm_nhwc_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(y), _ptr(weight), _ptr(bias), _ptr(ws),
+                                              ws.numel(), N, H * W, C, groups, samples, float(eps), int(silu), _stream())
+    _lib.check(st, "mc_groupnorm_nhwc_batched")
     if not want_stats:
         return y
     stats = torch.empty(N, groups, 2, dtype=torch.float32, device=x.device)
@@ -381,10 +400,11 @@ class GroupNormNHWCFn(torch.autograd.Function):
     """GroupNorm(+chan_bias)(+SiLU) on channels_last with the input gradient from csrc/norm_act.cu (weights frozen)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, chan_bias, groups: int, eps: float, silu: bool):
-        y, stats = groupnorm_nhwc(x, weight, bias, groups, eps, silu, chan_bias, want_stats=True)
+    def forward(ctx, x, weight, bias, chan_bias, groups: int, eps: float, silu: bool, samples: Optional[int] = None):
+        samples = _gn_samples if samples is None else int(samples)
+        y, stats = groupnorm_nhwc(x, weight, bias, groups, eps, silu, chan_bias, want_stats=True, samples=samples)
         ctx.save_for_backward(x, weight, bias, chan_bias, stats)
-        ctx.groups, ctx.silu = groups, silu
+        ctx.groups, ctx.silu, ctx.samples = groups, silu, samples
         return y
 
     @staticmethod
@@ -397,11 +417,11 @@ class GroupNormNHWCFn(torch.autograd.Function):
         weight, bias = _require_param(weight, "groupnorm weight", x, C), _require_param(bias, "groupnorm bias", x, C)
         dx = torch.empty_like(x)
         ws = _workspace(x, int(_lib.lib().mc_groupnorm_workspace_bytes(N, ctx.groups)), "bwd")
-        st = _lib.lib().mc_groupnorm_nhwc_bwd(_ptr(x), _ptr(chan_bias), fpr, _ptr(dz), _ptr(dx), _ptr(stats), _ptr(weight),
-                                              _ptr(bias), _ptr(ws), ws.numel(), N, H * W, C, ctx.groups, int(ctx.silu),
-                                              _stream())
-        _lib.check(st, "mc_groupnorm_nhwc_bwd")
-        return dx, None, None, None, None, None, None
+        st = _lib.lib().mc_groupnorm_nhwc_bwd_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(dz), _ptr(dx), _ptr(stats),
+                                                      _ptr(weight), _ptr(bias), _ptr(ws), ws.numel(), N, H * W, C,
+                                                      ctx.groups, ctx.samples, int(ctx.silu), _stream())
+        _lib.check(st, "mc_groupnorm_nhwc_bwd_batched")
+        return dx, None, None, None, None, None, None, None
 
 
 def layernorm(x: Tensor, weight: Tensor, bias: Tensor, eps: float, post_add: Optional[Tensor] = None,

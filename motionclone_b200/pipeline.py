@@ -69,7 +69,7 @@ class AnimationPipeline:
         self.vae, self.text_encoder, self.tokenizer = vae, text_encoder, tokenizer
         self.unet, self.scheduler, self.controlnet = unet, scheduler, controlnet
         self.vae_scale_factor = 8 if vae is None else 2 ** (len(vae.config.block_out_channels) - 1)
-        self.prompt_embeds: Optional[torch.Tensor] = None  # [2, 77, c]: row 0 uncond, row 1 cond (synthetic runs)
+        self.prompt_embeds: Optional[torch.Tensor] = None  # [2B, 77, c]: [uncond_1..B, cond_1..B] (synthetic runs)
         self.motion_representation_path = None
         self.motion_representation_dict = None
         self.input_config = None
@@ -95,7 +95,9 @@ class AnimationPipeline:
         self.__dict__.pop("_unet_graphs", None)
 
     def set_prompt_embeds(self, embeds: torch.Tensor):
-        """[2, 77, cross_attention_dim] = [uncond, cond] (the order _encode_prompt returns, :139 of the functions file)."""
+        """[2B, 77, cross_attention_dim] = [uncond_1..B, cond_1..B] for a batch of B samples (the order diffusers'
+        _encode_prompt returns, :139 of the functions file); B = 1 is [uncond, cond]. Motion extraction
+        (obtain_motion_representation) uses row 0."""
         self.prompt_embeds = embeds
         return self
 

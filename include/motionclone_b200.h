@@ -179,8 +179,9 @@ int mc_bias_residual_add(const void* a, const void* b, const void* bias, void* o
  * (csrc/groupnorm.cu): replaces InflatedGroupNorm + nonlinearity (models/resnet.py:21-29, :186-187, :197-204) and the
  * transformer input norms (models/attention.py:61,105; models/motion_module.py:112,145). Two launches: partial
  * (count, mean, M2) per split, folded into (mean, rstd) by the last CTA of each frame, then apply.
- * workspace: >= mc_groupnorm_workspace_bytes(N, G) bytes of device memory whose FIRST 4096 BYTES ARE ZERO on first use
- * (per-frame tickets; every call leaves them zero). One workspace per concurrently running stream.
+ * workspace: >= mc_groupnorm_workspace_bytes(N, G) bytes of device memory whose FIRST 8192 BYTES ARE ZERO on first use
+ * (per-frame and per-pool tickets; every call leaves them zero). One workspace per concurrently running stream. The size
+ * covers the per-frame and the frame-pooled calls below.
  */
 int64_t mc_groupnorm_workspace_bytes(int N, int G);
 /* chan_bias (nullable): fp16 [N / frames_per_bias_row, C] added to x before the statistics and the normalisation —
@@ -216,6 +217,23 @@ int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bias, int fram
                                   const void* stats, const void* gamma, const void* beta, void* workspace,
                                   int64_t workspace_bytes, int N, int HW, int C, int G, int samples, int fuse_silu,
                                   void* stream);
+/* Frame-pooled GroupNorm: one (mean, rstd) per group over each run of F = frames_per_stat consecutive frames (a "pool"),
+ * as torch.nn.GroupNorm computes on a 5-D [b, C, f, h, w] tensor with f = F (models/resnet.py:143-146, 162-165 and
+ * models/unet.py:244-247 when use_inflated_groupnorm=False). `samples` is the tiling unit of the _batched calls; a pool
+ * never straddles a sample: F >= 1, N % F == 0 and (N / samples) % F == 0, else MC_E_INVALID and nothing is launched.
+ * The pool's statistics are merged from per-frame (count, mean, M2) triples in frame order, so they depend on
+ * (F, samples, N / samples) only; F = 1 gives bitwise the results of mc_groupnorm_nhwc_batched / _bwd_batched.
+ * mc_groupnorm_nhwc_stats(workspace, stats, N, ...) after a pooled call returns [N, G, 2] in which the row of every
+ * frame holds its pool's (mean, rstd); rows f, f + 1, ..., f + F - 1 of a pool are equal, and rows 0, F, 2F, ... are
+ * the [N / F, G, 2] pool statistics. mc_groupnorm_nhwc_bwd_pooled takes that [N, G, 2] array as `stats`.
+ * Same workspace size and zero-ticket rule as above; N <= 1024 frames. */
+int mc_groupnorm_nhwc_pooled(const void* x, const void* chan_bias, int frames_per_bias_row, void* y, const void* gamma,
+                             const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW, int C, int G,
+                             int samples, int frames_per_stat, float eps, int fuse_silu, void* stream);
+int mc_groupnorm_nhwc_bwd_pooled(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz, void* dx,
+                                 const void* stats, const void* gamma, const void* beta, void* workspace,
+                                 int64_t workspace_bytes, int N, int HW, int C, int G, int samples, int frames_per_stat,
+                                 int fuse_silu, void* stream);
 int mc_layernorm_bwd(const void* x, const void* dy, void* dx, const void* gamma, const void* pre_bias, int64_t rows, int C,
                      float eps, void* stream);
 int mc_geglu_bwd(const void* in, const void* dout, void* din, int64_t T, int I, void* stream);

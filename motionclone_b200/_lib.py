@@ -26,7 +26,8 @@ _lib = None
 EXPORTS = ("mc_abi_version", "mc_last_error", "mc_launch_count", "mc_reset_launch_count", "mc_add_launch_count", "mc_temporal_attn_fwd",
            "mc_temporal_attn_bwd", "mc_top1_rows", "mc_motion_loss_fwd", "mc_motion_loss_bwd", "mc_cfg_ddim_step",
            "mc_add_noise", "mc_groupnorm_workspace_bytes", "mc_groupnorm_nhwc", "mc_layernorm", "mc_geglu", "mc_groupnorm_nhwc_stats", "mc_groupnorm_nhwc_bwd", "mc_layernorm_bwd",
-           "mc_groupnorm_nhwc_batched", "mc_groupnorm_nhwc_bwd_batched",
+           "mc_groupnorm_nhwc_batched", "mc_groupnorm_nhwc_bwd_batched", "mc_groupnorm_nhwc_pooled",
+           "mc_groupnorm_nhwc_bwd_pooled",
            "mc_geglu_bwd", "mc_bias_residual_add", "mc_cross_attn_fwd", "mc_cross_attn_bwd_dq",
            "mc_spatial_attn_fwd", "mc_spatial_attn_bwd", "mc_spatial_attn_bwd_workspace_bytes")
 
@@ -81,6 +82,12 @@ def lib() -> ctypes.CDLL:
     L.mc_groupnorm_nhwc_bwd_batched.restype = c_int
     L.mc_groupnorm_nhwc_bwd_batched.argtypes = [P, P, c_int, P, P, P, P, P, P, c_int64, c_int, c_int, c_int, c_int, c_int,
                                                 c_int, P]
+    L.mc_groupnorm_nhwc_pooled.restype = c_int
+    L.mc_groupnorm_nhwc_pooled.argtypes = [P, P, c_int, P, P, P, P, c_int64, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_float, c_int, P]
+    L.mc_groupnorm_nhwc_bwd_pooled.restype = c_int
+    L.mc_groupnorm_nhwc_bwd_pooled.argtypes = [P, P, c_int, P, P, P, P, P, P, c_int64, c_int, c_int, c_int, c_int, c_int,
+                                               c_int, c_int, P]
     L.mc_layernorm_bwd.restype = c_int
     L.mc_layernorm_bwd.argtypes = [P, P, P, P, P, c_int64, c_int, c_float, P]
     L.mc_geglu_bwd.restype = c_int

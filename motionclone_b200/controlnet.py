@@ -128,7 +128,8 @@ class SparseControlNetModel(nn.Module):
                 attn_num_head_channels=attention_head_dim[i] if attention_head_dim[i] is not None else out_c,
                 downsample_padding=downsample_padding,
                 use_motion_module=use_motion_module and (res in motion_module_resolutions),
-                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs))
+                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs,
+                use_inflated_groupnorm=True))  # per-frame norms whatever the UNet uses (sparse_controlnet.py:272)
             for _ in range(layers_per_block + (0 if final else 1)):
                 self.controlnet_down_blocks.append(zero_module(InflatedConv3d(out_c, out_c, kernel_size=1)))
         self.controlnet_mid_block = zero_module(InflatedConv3d(ch[-1], ch[-1], kernel_size=1))
@@ -137,7 +138,7 @@ class SparseControlNetModel(nn.Module):
             output_scale_factor=mid_block_scale_factor, cross_attention_dim=cross_attention_dim,
             attn_num_head_channels=num_attention_heads[-1],
             use_motion_module=use_motion_module and motion_module_mid_block, motion_module_type=motion_module_type,
-            motion_module_kwargs=motion_module_kwargs)
+            motion_module_kwargs=motion_module_kwargs, use_inflated_groupnorm=True)  # sparse_controlnet.py:310
         self._cond_cache = None
 
     @property

@@ -18,8 +18,14 @@
 //     only (shared memory, one warp per group, shuffles); ACROSS the splits of a frame the (count, mean, M2) partials are
 //     merged with Chan's formula (robust to |mean| >> std) by the LAST CTA of the frame (atomic ticket), which writes
 //     (mean, rstd): the apply pass reads 2 floats per group instead of re-folding the partials in every CTA.
-// Workspace layout (device memory, caller-owned): [4096 B tickets | N*G*2 floats finalised | N*S*G*3 floats partial].
-// The ticket region must be zero on first use; every call leaves it zero again.
+// Frame-pooled statistics (nn.GroupNorm on a 5-D `[b, C, f, h, w]` tensor: one mean / variance per group over F
+// consecutive frames) add a second level to that merge, in separate `_pooled` kernel instantiations: the last CTA of a
+// frame leaves the frame's (count, mean, M2) in its split-0 partial slot; the last frame of the pool (second ticket)
+// folds the F frame triples in frame order and writes the pool's (mean, rstd) into the row of each of its F frames, so
+// the apply and backward-apply kernels are the per-frame ones. The merge order depends on (F, S, PX) only, and at F = 1
+// every value is bitwise the per-frame one (one triple merged into an empty state, and a sum of one term, are exact).
+// Workspace layout (device memory, caller-owned): [8192 B tickets: 1024 per frame, 1024 per pool | N*G*2 floats
+// finalised | N*S*G*3 floats partial]. The ticket region must be zero on first use; every call leaves it zero again.
 #include <math.h>
 
 #include "mc_common.cuh"
@@ -31,7 +37,8 @@ union GVec8 {
   __half h[8];
 };
 
-constexpr int kGnTicketBytes = 4096;     // one uint32 per frame: N <= 1024
+constexpr int kGnMaxFrames = 1024;
+constexpr int kGnTicketBytes = 2 * kGnMaxFrames * 4;  // one uint32 per frame, then one per pool: N <= 1024
 constexpr int kGnMaxSplits = 128;
 constexpr int kGnTileBytes = 32 * 1024;  // shared-memory tile per CTA (forward: one tensor; backward: x and dz halves)
 constexpr int kGnHeader = 128;           // mbarrier
@@ -80,11 +87,12 @@ __device__ __forceinline__ void gn_fetch(uint8_t* buf, const __half* __restrict_
 // forward, pass 1: statistics. grid (N, S); CTA = pixels [HW*s/S, HW*(s+1)/S) of frame n in trips of PX pixels.
 // thread -> (vector column v = tid % V, pixel lane pl = tid / V).
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(512, 2) groupnorm_stats_kernel(const __half* __restrict__ x,
-                                                              const __half* __restrict__ chan_bias, int frames_per_row,
-                                                              float* __restrict__ partial, float* __restrict__ stats,
-                                                              unsigned* __restrict__ tickets, int HW, int C, int G, int S,
-                                                              int lanes, int PX, float eps) {
+// POOLED: statistics over the F = frames_per_stat consecutive frames of a pool (second merge level, see the top).
+template <bool POOLED>
+__device__ __forceinline__ void gn_stats_body(const __half* __restrict__ x, const __half* __restrict__ chan_bias,
+                                              int frames_per_row, float* __restrict__ partial, float* __restrict__ stats,
+                                              unsigned* __restrict__ tickets, int HW, int C, int G, int S, int lanes,
+                                              int PX, float eps, int frames_per_stat) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ unsigned s_ticket;
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);  // bar[0], bar[1]: one per stage
@@ -192,10 +200,53 @@ __global__ void __launch_bounds__(512, 2) groupnorm_stats_kernel(const __half* _
   for (int g = tid; g < G; g += NT) {
     float an = 0.f, amean = 0.f, am2 = 0.f;
     for (int k = 0; k < slices; ++k) chan_merge(an, amean, am2, f_n[k * G + g], f_mean[k * G + g], f_m2[k * G + g]);
-    stats[((int64_t)n * G + g) * 2] = amean;
-    stats[((int64_t)n * G + g) * 2 + 1] = rsqrtf(am2 / an + eps);
+    if (POOLED) {  // the frame's triple goes to its split-0 partial slot (already folded above)
+      float* out = partial + ((int64_t)n * S * G + g) * 3;
+      out[0] = an, out[1] = amean, out[2] = am2;
+    } else {
+      stats[((int64_t)n * G + g) * 2] = amean;
+      stats[((int64_t)n * G + g) * 2 + 1] = rsqrtf(am2 / an + eps);
+    }
   }
   if (tid == 0) tickets[n] = 0u;
+  if (!POOLED) return;
+  // ---- the last frame of the pool folds its F frame triples, in frame order, into (mean, rstd) ----
+  const int F = frames_per_stat, f0 = n - n % F;
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_ticket = atomicAdd(&tickets[kGnMaxFrames + n / F], 1u);
+  __syncthreads();
+  if (s_ticket != (unsigned)(F - 1)) return;
+  __threadfence();
+  for (int g = tid; g < G; g += NT) {
+    float an = 0.f, amean = 0.f, am2 = 0.f;
+    for (int f = f0; f < f0 + F; ++f) {
+      const float* p = partial + ((int64_t)f * S * G + g) * 3;
+      chan_merge(an, amean, am2, __ldcg(p), __ldcg(p + 1), __ldcg(p + 2));
+    }
+    const float rstd = rsqrtf(am2 / an + eps);
+    for (int f = f0; f < f0 + F; ++f) {
+      stats[((int64_t)f * G + g) * 2] = amean;
+      stats[((int64_t)f * G + g) * 2 + 1] = rstd;
+    }
+  }
+  if (tid == 0) tickets[kGnMaxFrames + n / F] = 0u;
+}
+
+__global__ void __launch_bounds__(512, 2) groupnorm_stats_kernel(const __half* __restrict__ x,
+                                                              const __half* __restrict__ chan_bias, int frames_per_row,
+                                                              float* __restrict__ partial, float* __restrict__ stats,
+                                                              unsigned* __restrict__ tickets, int HW, int C, int G, int S,
+                                                              int lanes, int PX, float eps) {
+  gn_stats_body<false>(x, chan_bias, frames_per_row, partial, stats, tickets, HW, C, G, S, lanes, PX, eps, 1);
+}
+
+__global__ void __launch_bounds__(512, 2) groupnorm_stats_pooled_kernel(
+    const __half* __restrict__ x, const __half* __restrict__ chan_bias, int frames_per_row, float* __restrict__ partial,
+    float* __restrict__ stats, unsigned* __restrict__ tickets, int HW, int C, int G, int S, int lanes, int PX, float eps,
+    int frames_per_stat) {
+  gn_stats_body<true>(x, chan_bias, frames_per_row, partial, stats, tickets, HW, C, G, S, lanes, PX, eps,
+                      frames_per_stat);
 }
 
 // forward, pass 2: y = a[c] * x + b[c] with a = rstd * gamma, b = beta - mean * a (ATen's fused-parameter form) [-> SiLU]
@@ -308,12 +359,14 @@ __device__ __forceinline__ void gn_bwd_coef(GnBwdCoef& k, const float* __restric
   }
 }
 
-template <bool SILU>
-__global__ void __launch_bounds__(512) groupnorm_bwd_reduce_kernel(
+// POOLED: the last CTA of a frame keeps the frame's raw sums; the last frame of the pool adds the F of them in frame
+// order and scales by 1 / (F * HW * cg). `stats` holds the pool's (mean, rstd) in the row of every frame.
+template <bool SILU, bool POOLED>
+__device__ __forceinline__ void gn_bwd_reduce_body(
     const __half* __restrict__ x, const __half* __restrict__ chan_bias, int frames_per_row, const __half* __restrict__ dz,
     const float* __restrict__ stats, const __half* __restrict__ gamma, const __half* __restrict__ beta,
     float* __restrict__ partial, float* __restrict__ ab, unsigned* __restrict__ tickets, int HW, int C, int G, int S,
-    int lanes, int PX) {
+    int lanes, int PX, int frames_per_stat) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ unsigned s_ticket;
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);  // bar[0], bar[1]
@@ -417,10 +470,57 @@ __global__ void __launch_bounds__(512) groupnorm_bwd_reduce_kernel(
   for (int g = tid; g < G; g += NT) {
     float ta = 0.f, tb = 0.f;
     for (int kk = 0; kk < slices; ++kk) ta += f_a[kk * G + g], tb += f_b[kk * G + g];
-    ab[((int64_t)n * G + g) * 2] = ta * inv_m;
-    ab[((int64_t)n * G + g) * 2 + 1] = tb * inv_m;
+    if (POOLED) {  // raw frame sums -> the frame's split-0 partial slot (already folded above)
+      float* out = partial + ((int64_t)n * S * G + g) * 2;
+      out[0] = ta, out[1] = tb;
+    } else {
+      ab[((int64_t)n * G + g) * 2] = ta * inv_m;
+      ab[((int64_t)n * G + g) * 2 + 1] = tb * inv_m;
+    }
   }
   if (tid == 0) tickets[n] = 0u;
+  if (!POOLED) return;
+  const int F = frames_per_stat, f0 = n - n % F;
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_ticket = atomicAdd(&tickets[kGnMaxFrames + n / F], 1u);
+  __syncthreads();
+  if (s_ticket != (unsigned)(F - 1)) return;
+  __threadfence();
+  const float inv_pool = 1.f / ((float)F * (float)HW * (float)cg);  // F = 1: the float inv_m is
+  for (int g = tid; g < G; g += NT) {
+    const float* p = partial + ((int64_t)f0 * S * G + g) * 2;
+    float ta = __ldcg(p), tb = __ldcg(p + 1);
+    for (int f = f0 + 1; f < f0 + F; ++f) {
+      p = partial + ((int64_t)f * S * G + g) * 2;
+      ta += __ldcg(p), tb += __ldcg(p + 1);
+    }
+    for (int f = f0; f < f0 + F; ++f) {
+      ab[((int64_t)f * G + g) * 2] = ta * inv_pool;
+      ab[((int64_t)f * G + g) * 2 + 1] = tb * inv_pool;
+    }
+  }
+  if (tid == 0) tickets[kGnMaxFrames + n / F] = 0u;
+}
+
+template <bool SILU>
+__global__ void __launch_bounds__(512) groupnorm_bwd_reduce_kernel(
+    const __half* __restrict__ x, const __half* __restrict__ chan_bias, int frames_per_row, const __half* __restrict__ dz,
+    const float* __restrict__ stats, const __half* __restrict__ gamma, const __half* __restrict__ beta,
+    float* __restrict__ partial, float* __restrict__ ab, unsigned* __restrict__ tickets, int HW, int C, int G, int S,
+    int lanes, int PX) {
+  gn_bwd_reduce_body<SILU, false>(x, chan_bias, frames_per_row, dz, stats, gamma, beta, partial, ab, tickets, HW, C, G, S,
+                                  lanes, PX, 1);
+}
+
+template <bool SILU>
+__global__ void __launch_bounds__(512) groupnorm_bwd_reduce_pooled_kernel(
+    const __half* __restrict__ x, const __half* __restrict__ chan_bias, int frames_per_row, const __half* __restrict__ dz,
+    const float* __restrict__ stats, const __half* __restrict__ gamma, const __half* __restrict__ beta,
+    float* __restrict__ partial, float* __restrict__ ab, unsigned* __restrict__ tickets, int HW, int C, int G, int S,
+    int lanes, int PX, int frames_per_stat) {
+  gn_bwd_reduce_body<SILU, true>(x, chan_bias, frames_per_row, dz, stats, gamma, beta, partial, ab, tickets, HW, C, G, S,
+                                 lanes, PX, frames_per_stat);
 }
 
 // pass 2: dx over the dz tile, in place, then one bulk store
@@ -567,9 +667,19 @@ static int gn_check(const char* what, int N, int HW, int C, int G, int samples) 
     set_error("%s: samples must be positive and divide N (got N=%d samples=%d)", what, N, samples);
     return MC_E_INVALID;
   }
-  if (C % 8 != 0 || C % G != 0 || C > 4096 || G > 128 || N > kGnTicketBytes / 4) {
+  if (C % 8 != 0 || C % G != 0 || C > 4096 || G > 128 || N > kGnMaxFrames) {
     set_error("%s: need C %% 8 == 0, C %% G == 0, C <= 4096, G <= 128, N <= 1024 (got N=%d C=%d G=%d)", what, N, C, G);
     return MC_E_UNSUPPORTED;
+  }
+  return MC_OK;
+}
+
+// a pool of F frames never straddles a tiling sample, so each sample's statistics stay its own
+static int gn_check_pool(const char* what, int N, int samples, int frames_per_stat) {
+  if (frames_per_stat < 1 || N % frames_per_stat != 0 || (N / samples) % frames_per_stat != 0) {
+    set_error("%s: frames_per_stat must be >= 1 and divide N / samples (got N=%d samples=%d frames_per_stat=%d)", what,
+              N, samples, frames_per_stat);
+    return MC_E_INVALID;
   }
   return MC_OK;
 }
@@ -594,22 +704,25 @@ extern "C" int64_t mc_groupnorm_workspace_bytes(int N, int G) {
   return mc::kGnTicketBytes + (int64_t)N * G * 2 * sizeof(float) + (int64_t)N * mc::kGnMaxSplits * G * 3 * sizeof(float);
 }
 
-extern "C" int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
-                                         const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes,
-                                         int N, int HW, int C, int G, int samples, float eps, int fuse_silu, void* stream) {
-  using namespace mc;
+namespace mc {
+
+// pool = 0: per-frame statistics (the original kernels); pool = F >= 1: statistics pooled over F frames
+static int gn_forward(const char* what, const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
+                      const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW, int C,
+                      int G, int samples, int pool, float eps, int fuse_silu, void* stream) {
   if (!x || !y || !gamma || !beta || !workspace) {
-    set_error("groupnorm_nhwc: null pointer");
+    set_error("%s: null pointer", what);
     return MC_E_INVALID;
   }
-  int rc = gn_check("groupnorm_nhwc", N, HW, C, G, samples);
+  int rc = gn_check(what, N, HW, C, G, samples);
   if (rc != MC_OK) return rc;
+  if (pool != 0 && (rc = gn_check_pool(what, N, samples, pool)) != MC_OK) return rc;
   if (chan_bias != nullptr && frames_per_bias_row <= 0) {
-    set_error("groupnorm_nhwc: frames_per_bias_row must be positive when chan_bias is given");
+    set_error("%s: frames_per_bias_row must be positive when chan_bias is given", what);
     return MC_E_INVALID;
   }
   if (workspace_bytes < mc_groupnorm_workspace_bytes(N, G)) {
-    set_error("groupnorm_nhwc: workspace too small (%lld < %lld bytes)", (long long)workspace_bytes,
+    set_error("%s: workspace too small (%lld < %lld bytes)", what, (long long)workspace_bytes,
               (long long)mc_groupnorm_workspace_bytes(N, G));
     return MC_E_INVALID;
   }
@@ -617,10 +730,17 @@ extern "C" int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, i
   const GnWorkspace w = gn_workspace(workspace, N, G);
   cudaStream_t st = (cudaStream_t)stream;
   const GnTiling T = gn_tiling(N / samples, HW, C, L.NT, 1, kGnTileBytes, 3);
-  gn_allow_smem(groupnorm_stats_kernel, T.smem);
-  groupnorm_stats_kernel<<<dim3(N, T.S), L.NT, T.smem, st>>>((const __half*)x, (const __half*)chan_bias,
-                                                             frames_per_bias_row, w.partial, w.finalised, w.tickets, HW, C,
-                                                             G, T.S, L.lanes, T.PX, eps);
+  if (pool != 0) {
+    gn_allow_smem(groupnorm_stats_pooled_kernel, T.smem);
+    groupnorm_stats_pooled_kernel<<<dim3(N, T.S), L.NT, T.smem, st>>>(
+        (const __half*)x, (const __half*)chan_bias, frames_per_bias_row, w.partial, w.finalised, w.tickets, HW, C, G, T.S,
+        L.lanes, T.PX, eps, pool);
+  } else {
+    gn_allow_smem(groupnorm_stats_kernel, T.smem);
+    groupnorm_stats_kernel<<<dim3(N, T.S), L.NT, T.smem, st>>>((const __half*)x, (const __half*)chan_bias,
+                                                               frames_per_bias_row, w.partial, w.finalised, w.tickets, HW,
+                                                               C, G, T.S, L.lanes, T.PX, eps);
+  }
   count_launch();
   rc = check_launch("groupnorm_stats");
   if (rc != MC_OK) return rc;
@@ -637,6 +757,27 @@ extern "C" int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, i
   }
   count_launch();
   return check_launch("groupnorm_apply");
+}
+
+}  // namespace mc
+
+extern "C" int mc_groupnorm_nhwc_batched(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
+                                         const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes,
+                                         int N, int HW, int C, int G, int samples, float eps, int fuse_silu, void* stream) {
+  return mc::gn_forward("groupnorm_nhwc", x, chan_bias, frames_per_bias_row, y, gamma, beta, workspace, workspace_bytes,
+                        N, HW, C, G, samples, 0, eps, fuse_silu, stream);
+}
+
+extern "C" int mc_groupnorm_nhwc_pooled(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
+                                        const void* gamma, const void* beta, void* workspace, int64_t workspace_bytes,
+                                        int N, int HW, int C, int G, int samples, int frames_per_stat, float eps,
+                                        int fuse_silu, void* stream) {
+  if (frames_per_stat < 1) {  // 0 would select the per-frame kernels in gn_forward
+    mc::set_error("groupnorm_nhwc_pooled: frames_per_stat must be >= 1 (got %d)", frames_per_stat);
+    return MC_E_INVALID;
+  }
+  return mc::gn_forward("groupnorm_nhwc_pooled", x, chan_bias, frames_per_bias_row, y, gamma, beta, workspace,
+                        workspace_bytes, N, HW, C, G, samples, frames_per_stat, eps, fuse_silu, stream);
 }
 
 extern "C" int mc_groupnorm_nhwc(const void* x, const void* chan_bias, int frames_per_bias_row, void* y,
@@ -663,23 +804,43 @@ extern "C" int mc_groupnorm_nhwc_stats(const void* workspace, void* stats, int N
   return MC_OK;
 }
 
-extern "C" int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bias, int frames_per_bias_row,
-                                             const void* dz, void* dx, const void* stats, const void* gamma,
-                                             const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW,
-                                             int C, int G, int samples, int fuse_silu, void* stream) {
-  using namespace mc;
+namespace mc {
+
+template <bool SILU>
+static void gn_launch_bwd_reduce(int pool, dim3 grid, int NT, int smem, cudaStream_t st, const __half* x,
+                                 const __half* cb, int fpr, const __half* dz, const float* stats, const __half* gamma,
+                                 const __half* beta, const GnWorkspace& w, int HW, int C, int G, const GnTiling& T,
+                                 int lanes) {
+  if (pool != 0) {
+    gn_allow_smem(groupnorm_bwd_reduce_pooled_kernel<SILU>, smem);
+    groupnorm_bwd_reduce_pooled_kernel<SILU><<<grid, NT, smem, st>>>(x, cb, fpr, dz, stats, gamma, beta, w.partial,
+                                                                     w.finalised, w.tickets, HW, C, G, T.S, lanes, T.PX,
+                                                                     pool);
+  } else {
+    gn_allow_smem(groupnorm_bwd_reduce_kernel<SILU>, smem);
+    groupnorm_bwd_reduce_kernel<SILU><<<grid, NT, smem, st>>>(x, cb, fpr, dz, stats, gamma, beta, w.partial, w.finalised,
+                                                              w.tickets, HW, C, G, T.S, lanes, T.PX);
+  }
+}
+
+// pool = 0: per-frame statistics; pool = F >= 1: `stats` and the gradient sums pooled over F frames
+static int gn_backward(const char* what, const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz,
+                       void* dx, const void* stats, const void* gamma, const void* beta, void* workspace,
+                       int64_t workspace_bytes, int N, int HW, int C, int G, int samples, int pool, int fuse_silu,
+                       void* stream) {
   if (!x || !dz || !dx || !stats || !gamma || !beta || !workspace) {
-    set_error("groupnorm_nhwc_bwd: null pointer");
+    set_error("%s: null pointer", what);
     return MC_E_INVALID;
   }
-  int rc = gn_check("groupnorm_nhwc_bwd", N, HW, C, G, samples);
+  int rc = gn_check(what, N, HW, C, G, samples);
   if (rc != MC_OK) return rc;
+  if (pool != 0 && (rc = gn_check_pool(what, N, samples, pool)) != MC_OK) return rc;
   if (chan_bias != nullptr && frames_per_bias_row <= 0) {
-    set_error("groupnorm_nhwc_bwd: frames_per_bias_row must be positive when chan_bias is given");
+    set_error("%s: frames_per_bias_row must be positive when chan_bias is given", what);
     return MC_E_INVALID;
   }
   if (workspace_bytes < mc_groupnorm_workspace_bytes(N, G)) {
-    set_error("groupnorm_nhwc_bwd: workspace too small");
+    set_error("%s: workspace too small", what);
     return MC_E_INVALID;
   }
   const GnLaunch L = gn_launch(C);
@@ -688,35 +849,51 @@ extern "C" int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bia
   const GnTiling T = gn_tiling(N / samples, HW, C, L.NT, 2, kGnTileBytes / 2, 2);
   const __half *xp = (const __half*)x, *cbp = (const __half*)chan_bias, *dzp = (const __half*)dz;
   const __half *gp = (const __half*)gamma, *bp = (const __half*)beta;
-  if (fuse_silu) {
-    gn_allow_smem(groupnorm_bwd_reduce_kernel<true>, T.smem);
-    groupnorm_bwd_reduce_kernel<true><<<dim3(N, T.S), L.NT, T.smem, st>>>(xp, cbp, frames_per_bias_row, dzp,
-                                                                          (const float*)stats, gp, bp, w.partial,
-                                                                          w.finalised, w.tickets, HW, C, G, T.S, L.lanes,
-                                                                          T.PX);
-  } else {
-    gn_allow_smem(groupnorm_bwd_reduce_kernel<false>, T.smem);
-    groupnorm_bwd_reduce_kernel<false><<<dim3(N, T.S), L.NT, T.smem, st>>>(xp, cbp, frames_per_bias_row, dzp,
-                                                                           (const float*)stats, gp, bp, w.partial,
-                                                                           w.finalised, w.tickets, HW, C, G, T.S, L.lanes,
-                                                                           T.PX);
-  }
+  const float* sp = (const float*)stats;
+  if (fuse_silu)
+    gn_launch_bwd_reduce<true>(pool, dim3(N, T.S), L.NT, T.smem, st, xp, cbp, frames_per_bias_row, dzp, sp, gp, bp, w, HW,
+                               C, G, T, L.lanes);
+  else
+    gn_launch_bwd_reduce<false>(pool, dim3(N, T.S), L.NT, T.smem, st, xp, cbp, frames_per_bias_row, dzp, sp, gp, bp, w,
+                                HW, C, G, T, L.lanes);
   count_launch();
   rc = check_launch("groupnorm_bwd_reduce");
   if (rc != MC_OK) return rc;
   if (fuse_silu) {
     gn_allow_smem(groupnorm_bwd_apply_kernel<true>, T.smem);
     groupnorm_bwd_apply_kernel<true><<<dim3(N, T.S), L.NT, T.smem, st>>>(xp, cbp, frames_per_bias_row, dzp, (__half*)dx,
-                                                                         (const float*)stats, w.finalised, gp, bp, HW, C, G,
-                                                                         T.S, L.lanes, T.PX);
+                                                                         sp, w.finalised, gp, bp, HW, C, G, T.S, L.lanes,
+                                                                         T.PX);
   } else {
     gn_allow_smem(groupnorm_bwd_apply_kernel<false>, T.smem);
     groupnorm_bwd_apply_kernel<false><<<dim3(N, T.S), L.NT, T.smem, st>>>(xp, cbp, frames_per_bias_row, dzp, (__half*)dx,
-                                                                          (const float*)stats, w.finalised, gp, bp, HW, C,
-                                                                          G, T.S, L.lanes, T.PX);
+                                                                          sp, w.finalised, gp, bp, HW, C, G, T.S, L.lanes,
+                                                                          T.PX);
   }
   count_launch();
   return check_launch("groupnorm_bwd_apply");
+}
+
+}  // namespace mc
+
+extern "C" int mc_groupnorm_nhwc_bwd_batched(const void* x, const void* chan_bias, int frames_per_bias_row,
+                                             const void* dz, void* dx, const void* stats, const void* gamma,
+                                             const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW,
+                                             int C, int G, int samples, int fuse_silu, void* stream) {
+  return mc::gn_backward("groupnorm_nhwc_bwd", x, chan_bias, frames_per_bias_row, dz, dx, stats, gamma, beta, workspace,
+                         workspace_bytes, N, HW, C, G, samples, 0, fuse_silu, stream);
+}
+
+extern "C" int mc_groupnorm_nhwc_bwd_pooled(const void* x, const void* chan_bias, int frames_per_bias_row,
+                                            const void* dz, void* dx, const void* stats, const void* gamma,
+                                            const void* beta, void* workspace, int64_t workspace_bytes, int N, int HW,
+                                            int C, int G, int samples, int frames_per_stat, int fuse_silu, void* stream) {
+  if (frames_per_stat < 1) {
+    mc::set_error("groupnorm_nhwc_bwd_pooled: frames_per_stat must be >= 1 (got %d)", frames_per_stat);
+    return MC_E_INVALID;
+  }
+  return mc::gn_backward("groupnorm_nhwc_bwd_pooled", x, chan_bias, frames_per_bias_row, dz, dx, stats, gamma, beta,
+                         workspace, workspace_bytes, N, HW, C, G, samples, frames_per_stat, fuse_silu, stream);
 }
 
 extern "C" int mc_groupnorm_nhwc_bwd(const void* x, const void* chan_bias, int frames_per_bias_row, const void* dz,

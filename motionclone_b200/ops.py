@@ -349,9 +349,9 @@ def _require_param(t: Tensor, name: str, like: Tensor, numel: int) -> Tensor:
 
 
 def _workspace(x: Tensor, need: int, role: str = "fwd") -> Tensor:
-    """Per (device, stream, role) scratch for the GroupNorm kernels. Zero-initialised: its first 4 KB are the per-frame
-    tickets of the last-CTA reduction, which the kernels leave at zero (include/motionclone_b200.h). Forward and backward
-    use different buffers (the forward's finalised statistics are copied out for the backward)."""
+    """Per (device, stream, role) scratch for the GroupNorm kernels. Zero-initialised: its first 8 KB are the per-frame
+    and per-pool tickets of the last-CTA reductions, which the kernels leave at zero (include/motionclone_b200.h).
+    Forward and backward use different buffers (the forward's finalised statistics are copied out for the backward)."""
     key = (x.device, torch.cuda.current_stream().cuda_stream, role)
     ws = _gn_workspace.get(key)
     if ws is None or ws.numel() < need:
@@ -371,11 +371,14 @@ def _check_chan_bias(x: Tensor, chan_bias: Optional[Tensor]):
 
 
 def groupnorm_nhwc(x: Tensor, weight: Tensor, bias: Tensor, groups: int, eps: float, silu: bool = False,
-                   chan_bias: Optional[Tensor] = None, want_stats: bool = False, samples: Optional[int] = None):
+                   chan_bias: Optional[Tensor] = None, want_stats: bool = False, samples: Optional[int] = None,
+                   frames_per_stat: Optional[int] = None):
     """x: [N, C, h, w] in channels_last (physically [N, h, w, C]); returns the same format. `chan_bias` [NB, C]
     (N % NB == 0) is added to x first, row n // (N // NB) — the resnet's time-embedding add folded in.
     `want_stats` also returns (mean, rstd) [N, groups, 2] fp32 for the backward. `samples` (N % samples == 0; default:
-    the enclosing `batch_samples`, else 1) makes the result of each sample independent of the others in the batch."""
+    the enclosing `batch_samples`, else 1) makes the result of each sample independent of the others in the batch.
+    `frames_per_stat` F pools the statistics over each run of F consecutive frames (nn.GroupNorm on `[b, C, F, h, w]`;
+    F must divide N / samples); the stats row of every frame then holds its pool's values. None: per frame."""
     _require(x, "x")
     if x.dim() != 4 or not x.is_contiguous(memory_format=torch.channels_last):
         raise ValueError("groupnorm_nhwc expects a 4-D channels_last tensor")
@@ -385,9 +388,16 @@ def groupnorm_nhwc(x: Tensor, weight: Tensor, bias: Tensor, groups: int, eps: fl
     weight, bias = _require_param(weight, "groupnorm weight", x, C), _require_param(bias, "groupnorm bias", x, C)
     y = torch.empty_like(x)  # preserves channels_last
     ws = _workspace(x, int(_lib.lib().mc_groupnorm_workspace_bytes(N, groups)))
-    st = _lib.lib().mc_groupnorm_nhwc_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(y), _ptr(weight), _ptr(bias), _ptr(ws),
-                                              ws.numel(), N, H * W, C, groups, samples, float(eps), int(silu), _stream())
-    _lib.check(st, "mc_groupnorm_nhwc_batched")
+    if frames_per_stat is None:
+        st = _lib.lib().mc_groupnorm_nhwc_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(y), _ptr(weight), _ptr(bias),
+                                                  _ptr(ws), ws.numel(), N, H * W, C, groups, samples, float(eps),
+                                                  int(silu), _stream())
+        _lib.check(st, "mc_groupnorm_nhwc_batched")
+    else:
+        st = _lib.lib().mc_groupnorm_nhwc_pooled(_ptr(x), _ptr(chan_bias), fpr, _ptr(y), _ptr(weight), _ptr(bias),
+                                                 _ptr(ws), ws.numel(), N, H * W, C, groups, samples,
+                                                 int(frames_per_stat), float(eps), int(silu), _stream())
+        _lib.check(st, "mc_groupnorm_nhwc_pooled")
     if not want_stats:
         return y
     stats = torch.empty(N, groups, 2, dtype=torch.float32, device=x.device)
@@ -400,11 +410,13 @@ class GroupNormNHWCFn(torch.autograd.Function):
     """GroupNorm(+chan_bias)(+SiLU) on channels_last with the input gradient from csrc/norm_act.cu (weights frozen)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, chan_bias, groups: int, eps: float, silu: bool, samples: Optional[int] = None):
+    def forward(ctx, x, weight, bias, chan_bias, groups: int, eps: float, silu: bool, samples: Optional[int] = None,
+                frames_per_stat: Optional[int] = None):
         samples = _gn_samples if samples is None else int(samples)
-        y, stats = groupnorm_nhwc(x, weight, bias, groups, eps, silu, chan_bias, want_stats=True, samples=samples)
+        y, stats = groupnorm_nhwc(x, weight, bias, groups, eps, silu, chan_bias, want_stats=True, samples=samples,
+                                  frames_per_stat=frames_per_stat)
         ctx.save_for_backward(x, weight, bias, chan_bias, stats)
-        ctx.groups, ctx.silu, ctx.samples = groups, silu, samples
+        ctx.groups, ctx.silu, ctx.samples, ctx.frames_per_stat = groups, silu, samples, frames_per_stat
         return y
 
     @staticmethod
@@ -417,11 +429,18 @@ class GroupNormNHWCFn(torch.autograd.Function):
         weight, bias = _require_param(weight, "groupnorm weight", x, C), _require_param(bias, "groupnorm bias", x, C)
         dx = torch.empty_like(x)
         ws = _workspace(x, int(_lib.lib().mc_groupnorm_workspace_bytes(N, ctx.groups)), "bwd")
-        st = _lib.lib().mc_groupnorm_nhwc_bwd_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(dz), _ptr(dx), _ptr(stats),
-                                                      _ptr(weight), _ptr(bias), _ptr(ws), ws.numel(), N, H * W, C,
-                                                      ctx.groups, ctx.samples, int(ctx.silu), _stream())
-        _lib.check(st, "mc_groupnorm_nhwc_bwd_batched")
-        return dx, None, None, None, None, None, None, None
+        if ctx.frames_per_stat is None:
+            st = _lib.lib().mc_groupnorm_nhwc_bwd_batched(_ptr(x), _ptr(chan_bias), fpr, _ptr(dz), _ptr(dx), _ptr(stats),
+                                                          _ptr(weight), _ptr(bias), _ptr(ws), ws.numel(), N, H * W, C,
+                                                          ctx.groups, ctx.samples, int(ctx.silu), _stream())
+            _lib.check(st, "mc_groupnorm_nhwc_bwd_batched")
+        else:
+            st = _lib.lib().mc_groupnorm_nhwc_bwd_pooled(_ptr(x), _ptr(chan_bias), fpr, _ptr(dz), _ptr(dx), _ptr(stats),
+                                                         _ptr(weight), _ptr(bias), _ptr(ws), ws.numel(), N, H * W, C,
+                                                         ctx.groups, ctx.samples, int(ctx.frames_per_stat),
+                                                         int(ctx.silu), _stream())
+            _lib.check(st, "mc_groupnorm_nhwc_bwd_pooled")
+        return dx, None, None, None, None, None, None, None, None
 
 
 def layernorm(x: Tensor, weight: Tensor, bias: Tensor, eps: float, post_add: Optional[Tensor] = None,

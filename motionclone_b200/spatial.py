@@ -95,13 +95,30 @@ class GroupNormNHWC(nn.GroupNorm):
 
     def forward(self, x, silu: bool = False, chan_bias=None):
         """chan_bias [NB, C]: per-(batch row, channel) bias added to x first (the resnet's `+ temb`)."""
+        return self._norm(x, silu, chan_bias, None)
+
+    def _norm(self, x, silu, chan_bias, frames_per_stat):
         _need_kernels(x, "GroupNorm")
         if not (x.dim() == 4 and x.shape[1] % 8 == 0 and x.shape[1] <= 4096
                 and x.is_contiguous(memory_format=torch.channels_last) and _frozen(self.weight, self.bias, chan_bias)):
             raise NotImplementedError("GroupNorm kernel: 4-D channels_last input, C % 8 == 0, C <= 4096, frozen weights")
         if torch.is_grad_enabled() and x.requires_grad:
-            return ops.GroupNormNHWCFn.apply(x, self.weight, self.bias, chan_bias, self.num_groups, self.eps, silu)
-        return ops.groupnorm_nhwc(x, self.weight, self.bias, self.num_groups, self.eps, silu, chan_bias)
+            return ops.GroupNormNHWCFn.apply(x, self.weight, self.bias, chan_bias, self.num_groups, self.eps, silu, None,
+                                             frames_per_stat)
+        return ops.groupnorm_nhwc(x, self.weight, self.bias, self.num_groups, self.eps, silu, chan_bias,
+                                  frames_per_stat=frames_per_stat)
+
+
+class FramePooledGroupNormNHWC(GroupNormNHWC):
+    """GroupNormNHWC whose statistics are pooled over the `frames` consecutive frames of each batch element of a
+    `[(b f), C, h, w]` activation: torch.nn.GroupNorm applied to the 5-D `[b, C, f, h, w]` tensor (models/resnet.py:
+    143-146, 162-165 and models/unet.py:244-247 when use_inflated_groupnorm=False). Same parameters and state-dict keys
+    as nn.GroupNorm; the caller passes the frame count."""
+
+    def forward(self, x, silu: bool = False, chan_bias=None, frames: Optional[int] = None):
+        if frames is None or int(frames) < 1 or x.shape[0] % int(frames):
+            raise ValueError(f"frame-pooled GroupNorm needs the frame count f >= 1 dividing {x.shape[0]}, got {frames}")
+        return self._norm(x, silu, chan_bias, int(frames))
 
 
 class GEGLU(nn.Module):

@@ -39,6 +39,11 @@ UNET_SD15_CONFIG = dict(
 UNET_TINY_CONFIG = dict(UNET_SD15_CONFIG, sample_size=16, block_out_channels=(64, 128, 256, 256),
                         cross_attention_dim=96)
 
+# The reference's default GroupNorm mode (unet.py:80, resnet.py:126): resnet and output norms pool their statistics over
+# the frames of each batch element (torch.nn.GroupNorm on the 5-D tensor); the state dict is the same.
+UNET_SD15_POOLED_GN_CONFIG = dict(UNET_SD15_CONFIG, use_inflated_groupnorm=False)
+UNET_TINY_POOLED_GN_CONFIG = dict(UNET_TINY_CONFIG, use_inflated_groupnorm=False)
+
 # configs/model_config/model_config.yaml:17-21
 NOISE_SCHEDULER_KWARGS = dict(beta_start=0.00085, beta_end=0.012, beta_schedule="linear", steps_offset=1,
                               clip_sample=False)

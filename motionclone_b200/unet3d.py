@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from .spatial import GroupNormNHWC, Transformer3DModel
+from .spatial import FramePooledGroupNormNHWC, GroupNormNHWC, Transformer3DModel
 from .temporal import get_motion_module
 
 CL = torch.channels_last
@@ -61,6 +61,18 @@ class InflatedGroupNorm(GroupNormNHWC):
             return super().forward(x, silu, chan_bias)
         x4, bf = _fold5(x)
         return _unfold5(super().forward(x4, silu, chan_bias), bf)
+
+
+class FramePooledGroupNorm(FramePooledGroupNormNHWC):
+    """torch.nn.GroupNorm on the 5-D tensor (resnet.py:143-146, 162-165, unet.py:244-247 with
+    use_inflated_groupnorm=False): statistics pooled over the f frames of each batch element. 4-D channels_last
+    `[(b f), C, h, w]` inputs take the NHWC kernel with the caller's frame count."""
+
+    def forward(self, x, silu: bool = False, chan_bias=None, frames=None):
+        if x.dim() == 4:
+            return super().forward(x, silu, chan_bias, frames)
+        x4, bf = _fold5(x)
+        return _unfold5(super().forward(x4, silu, chan_bias, bf[1]), bf)
 
 
 class Upsample3D(nn.Module):
@@ -110,17 +122,16 @@ class ResnetBlock3D(nn.Module):
         super().__init__()
         if time_embedding_norm != "default" or non_linearity not in ("swish", "silu"):
             raise NotImplementedError("scale_shift / mish are never configured by the reference")
-        if not use_inflated_groupnorm:
-            raise NotImplementedError("use_inflated_groupnorm=False (resnet.py:143-165: GroupNorm statistics pooled across "
-                                      "frames) is not implemented")
         out_channels = in_channels if out_channels is None else out_channels
         self.in_channels, self.out_channels = in_channels, out_channels
         self.time_embedding_norm, self.output_scale_factor = time_embedding_norm, output_scale_factor
         groups_out = groups if groups_out is None else groups_out
-        self.norm1 = InflatedGroupNorm(num_groups=groups, num_channels=in_channels, eps=eps, affine=True)
+        self.use_inflated_groupnorm = use_inflated_groupnorm
+        norm = InflatedGroupNorm if use_inflated_groupnorm else FramePooledGroupNorm
+        self.norm1 = norm(num_groups=groups, num_channels=in_channels, eps=eps, affine=True)
         self.conv1 = InflatedConv3d(in_channels, out_channels, kernel_size=3, stride=1, padding=1)
         self.time_emb_proj = nn.Linear(temb_channels, out_channels) if temb_channels is not None else None
-        self.norm2 = InflatedGroupNorm(num_groups=groups_out, num_channels=out_channels, eps=eps, affine=True)
+        self.norm2 = norm(num_groups=groups_out, num_channels=out_channels, eps=eps, affine=True)
         self.dropout = nn.Dropout(dropout)
         self.conv2 = InflatedConv3d(out_channels, out_channels, kernel_size=3, stride=1, padding=1)
         self.nonlinearity = F.silu
@@ -138,13 +149,15 @@ class ResnetBlock3D(nn.Module):
 
     def forward(self, x, temb_act):
         """x `[(b f), C, h, w]`; temb_act `[b, temb_channels]` = SiLU(time embedding) (resnet.py:192 applies the SiLU
-        in every block; it is hoisted). The projection runs once per batch element and is broadcast over frames."""
+        in every block; it is hoisted). The projection runs once per batch element and is broadcast over frames.
+        Frame-pooled norms take f = (b f) / b frames per batch element."""
+        fk = {} if self.use_inflated_groupnorm else {"frames": x.shape[0] // temb_act.shape[0]}
         if self._fused_ok(x):
             # conv biases never get their own elementwise pass: conv1's joins the time embedding inside norm2's
             # channel bias, conv2's (+ the shortcut conv's) joins the residual add (one launch: csrc/elementwise.cu)
-            h = F.conv2d(self.norm1(x, silu=True), self.conv1.weight, None, 1, 1)
+            h = F.conv2d(self.norm1(x, silu=True, **fk), self.conv1.weight, None, 1, 1)
             t = self.time_emb_proj(temb_act) + self.conv1.bias
-            h = F.conv2d(self.dropout(self.norm2(h, silu=True, chan_bias=t)), self.conv2.weight, None, 1, 1)
+            h = F.conv2d(self.dropout(self.norm2(h, silu=True, chan_bias=t, **fk)), self.conv2.weight, None, 1, 1)
             if self.keep_hidden_state:
                 self.record_hidden_state = h
             bias = self.conv2.bias
@@ -154,10 +167,10 @@ class ResnetBlock3D(nn.Module):
             if torch.is_grad_enabled() and (h.requires_grad or x.requires_grad):
                 return ops.BiasResidualAddFn.apply(h, x, bias)
             return ops.bias_residual_add(h, x, bias)
-        h = self.conv1(self.norm1(x, silu=True))
+        h = self.conv1(self.norm1(x, silu=True, **fk))
         t = self.time_emb_proj(temb_act) if self.time_emb_proj is not None else None
         # `hidden_states + temb` (resnet.py:194-195) is folded into norm2 (broadcast over frames and pixels)
-        h = self.conv2(self.dropout(self.norm2(h, silu=True, chan_bias=t)))
+        h = self.conv2(self.dropout(self.norm2(h, silu=True, chan_bias=t, **fk)))
         if self.keep_hidden_state:
             self.record_hidden_state = h
         if self.conv_shortcut is not None:
@@ -173,9 +186,9 @@ class _BlockBase(nn.Module):
     gradient_checkpointing = False
 
     @staticmethod
-    def _resnet(cin, cout, temb, eps, groups, scale=1.0):
+    def _resnet(cin, cout, temb, eps, groups, inflated_gn, scale=1.0):
         return ResnetBlock3D(in_channels=cin, out_channels=cout, temb_channels=temb, eps=eps, groups=groups,
-                             output_scale_factor=scale, use_inflated_groupnorm=True)
+                             output_scale_factor=scale, use_inflated_groupnorm=inflated_gn)
 
     @staticmethod
     def _attn(heads, cout, cross_dim, groups, **kw):
@@ -194,11 +207,13 @@ class CrossAttnDownBlock3D(_BlockBase):
 
     def __init__(self, in_channels, out_channels, temb_channels, num_layers=1, resnet_eps=1e-6, resnet_groups=32,
                  attn_num_head_channels=1, cross_attention_dim=1280, downsample_padding=1, add_downsample=True,
-                 use_motion_module=None, motion_module_type=None, motion_module_kwargs=None, **unused):
+                 use_motion_module=None, motion_module_type=None, motion_module_kwargs=None,
+                 use_inflated_groupnorm=False, **unused):
         super().__init__()
         self.attn_num_head_channels = attn_num_head_channels
         self.resnets = nn.ModuleList([self._resnet(in_channels if i == 0 else out_channels, out_channels, temb_channels,
-                                                   resnet_eps, resnet_groups) for i in range(num_layers)])
+                                                   resnet_eps, resnet_groups, use_inflated_groupnorm)
+                                      for i in range(num_layers)])
         self.attentions = nn.ModuleList([self._attn(attn_num_head_channels, out_channels, cross_attention_dim,
                                                     resnet_groups) for _ in range(num_layers)])
         self.motion_modules = nn.ModuleList([self._mm(out_channels, use_motion_module, motion_module_type,
@@ -228,10 +243,11 @@ class DownBlock3D(_BlockBase):
 
     def __init__(self, in_channels, out_channels, temb_channels, num_layers=1, resnet_eps=1e-6, resnet_groups=32,
                  add_downsample=True, downsample_padding=1, use_motion_module=None, motion_module_type=None,
-                 motion_module_kwargs=None, **unused):
+                 motion_module_kwargs=None, use_inflated_groupnorm=False, **unused):
         super().__init__()
         self.resnets = nn.ModuleList([self._resnet(in_channels if i == 0 else out_channels, out_channels, temb_channels,
-                                                   resnet_eps, resnet_groups) for i in range(num_layers)])
+                                                   resnet_eps, resnet_groups, use_inflated_groupnorm)
+                                      for i in range(num_layers)])
         self.motion_modules = nn.ModuleList([self._mm(out_channels, use_motion_module, motion_module_type,
                                                       motion_module_kwargs) for _ in range(num_layers)])
         self.downsamplers = nn.ModuleList([Downsample3D(out_channels, use_conv=True, out_channels=out_channels,
@@ -258,12 +274,13 @@ class UNetMidBlock3DCrossAttn(_BlockBase):
 
     def __init__(self, in_channels, temb_channels, num_layers=1, resnet_eps=1e-6, resnet_groups=32,
                  attn_num_head_channels=1, output_scale_factor=1.0, cross_attention_dim=1280, use_motion_module=None,
-                 motion_module_type=None, motion_module_kwargs=None, **unused):
+                 motion_module_type=None, motion_module_kwargs=None, use_inflated_groupnorm=False, **unused):
         super().__init__()
         self.attn_num_head_channels = attn_num_head_channels
         resnet_groups = resnet_groups if resnet_groups is not None else min(in_channels // 4, 32)
         self.resnets = nn.ModuleList([self._resnet(in_channels, in_channels, temb_channels, resnet_eps, resnet_groups,
-                                                   output_scale_factor) for _ in range(num_layers + 1)])
+                                                   use_inflated_groupnorm, output_scale_factor)
+                                      for _ in range(num_layers + 1)])
         self.attentions = nn.ModuleList([self._attn(attn_num_head_channels, in_channels, cross_attention_dim,
                                                     resnet_groups) for _ in range(num_layers)])
         self.motion_modules = nn.ModuleList([self._mm(in_channels, use_motion_module, motion_module_type,
@@ -285,14 +302,16 @@ class CrossAttnUpBlock3D(_BlockBase):
 
     def __init__(self, in_channels, out_channels, prev_output_channel, temb_channels, num_layers=1, resnet_eps=1e-6,
                  resnet_groups=32, attn_num_head_channels=1, cross_attention_dim=1280, add_upsample=True,
-                 use_motion_module=None, motion_module_type=None, motion_module_kwargs=None, **unused):
+                 use_motion_module=None, motion_module_type=None, motion_module_kwargs=None,
+                 use_inflated_groupnorm=False, **unused):
         super().__init__()
         self.attn_num_head_channels = attn_num_head_channels
         resnets = []
         for i in range(num_layers):
             skip = in_channels if i == num_layers - 1 else out_channels
             cin = prev_output_channel if i == 0 else out_channels
-            resnets.append(self._resnet(cin + skip, out_channels, temb_channels, resnet_eps, resnet_groups))
+            resnets.append(self._resnet(cin + skip, out_channels, temb_channels, resnet_eps, resnet_groups,
+                                        use_inflated_groupnorm))
         self.resnets = nn.ModuleList(resnets)
         self.attentions = nn.ModuleList([self._attn(attn_num_head_channels, out_channels, cross_attention_dim,
                                                     resnet_groups) for _ in range(num_layers)])
@@ -321,13 +340,14 @@ class UpBlock3D(_BlockBase):
 
     def __init__(self, in_channels, prev_output_channel, out_channels, temb_channels, num_layers=1, resnet_eps=1e-6,
                  resnet_groups=32, add_upsample=True, use_motion_module=None, motion_module_type=None,
-                 motion_module_kwargs=None, **unused):
+                 motion_module_kwargs=None, use_inflated_groupnorm=False, **unused):
         super().__init__()
         resnets = []
         for i in range(num_layers):
             skip = in_channels if i == num_layers - 1 else out_channels
             cin = prev_output_channel if i == 0 else out_channels
-            resnets.append(self._resnet(cin + skip, out_channels, temb_channels, resnet_eps, resnet_groups))
+            resnets.append(self._resnet(cin + skip, out_channels, temb_channels, resnet_eps, resnet_groups,
+                                        use_inflated_groupnorm))
         self.resnets = nn.ModuleList(resnets)
         self.motion_modules = nn.ModuleList([self._mm(out_channels, use_motion_module, motion_module_type,
                                                       motion_module_kwargs) for _ in range(num_layers)])
@@ -441,12 +461,6 @@ class UNet3DConditionModel(nn.Module):
                 or use_linear_projection or unet_use_cross_frame_attention or unet_use_temporal_attention \
                 or center_input_sample or only_cross_attention not in (False, (False,) * 4, [False] * 4):
             raise NotImplementedError("configuration outside the reference's live path (SURVEY.md appendix A)")
-        if not use_inflated_groupnorm:
-            # resnet.py:143-165 / unet.py:244 use torch.nn.GroupNorm on the 5-D tensor in that mode (statistics pooled
-            # across frames); every shipped config sets use_inflated_groupnorm: true (model_config.yaml:2) and only the
-            # per-frame form is implemented here - refuse instead of silently computing different numbers
-            raise NotImplementedError("use_inflated_groupnorm=False (cross-frame GroupNorm statistics) is not implemented; "
-                                      "all shipped configs use the inflated (per-frame) GroupNorm")
         motion_module_kwargs = dict(motion_module_kwargs or {})
         self.sample_size = sample_size
         self.input_config = None  # set by the driver (t2v_video_sample.py:69)
@@ -470,7 +484,8 @@ class UNet3DConditionModel(nn.Module):
                 cross_attention_dim=cross_attention_dim, attn_num_head_channels=attention_head_dim[i],
                 downsample_padding=downsample_padding,
                 use_motion_module=use_motion_module and (res in motion_module_resolutions) and not motion_module_decoder_only,
-                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs))
+                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs,
+                use_inflated_groupnorm=use_inflated_groupnorm))
 
         if mid_block_type != "UNetMidBlock3DCrossAttn":
             raise ValueError(f"unknown mid_block_type : {mid_block_type}")
@@ -479,7 +494,7 @@ class UNet3DConditionModel(nn.Module):
             output_scale_factor=mid_block_scale_factor, cross_attention_dim=cross_attention_dim,
             attn_num_head_channels=attention_head_dim[-1],
             use_motion_module=use_motion_module and motion_module_mid_block, motion_module_type=motion_module_type,
-            motion_module_kwargs=motion_module_kwargs)
+            motion_module_kwargs=motion_module_kwargs, use_inflated_groupnorm=use_inflated_groupnorm)
 
         self.num_upsamplers = 0
         self.up_blocks = nn.ModuleList()
@@ -498,9 +513,12 @@ class UNet3DConditionModel(nn.Module):
                 resnet_eps=norm_eps, resnet_groups=norm_num_groups, cross_attention_dim=cross_attention_dim,
                 attn_num_head_channels=rheads[i],
                 use_motion_module=use_motion_module and (res in motion_module_resolutions),
-                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs))
+                motion_module_type=motion_module_type, motion_module_kwargs=motion_module_kwargs,
+                use_inflated_groupnorm=use_inflated_groupnorm))
 
-        self.conv_norm_out = InflatedGroupNorm(num_channels=ch[0], num_groups=norm_num_groups, eps=norm_eps)
+        # resnet norms and the output norm only: the transformer and motion-module norms stay per frame in both modes
+        norm_out = InflatedGroupNorm if use_inflated_groupnorm else FramePooledGroupNorm
+        self.conv_norm_out = norm_out(num_channels=ch[0], num_groups=norm_num_groups, eps=norm_eps)
         self.conv_act = nn.SiLU()
         self.conv_out = InflatedConv3d(ch[0], out_channels, kernel_size=3, padding=1)
 
@@ -587,6 +605,7 @@ class UNet3DConditionModel(nn.Module):
                 with torch.no_grad():  # :629
                     x = blk(x, res, temb, encoder_hidden_states, f, upsample_size=size)
 
-        x = self.conv_out(self.conv_norm_out(x, silu=True))  # conv_act (SiLU) fused into the norm
+        fk = {} if self.config.use_inflated_groupnorm else {"frames": f}
+        x = self.conv_out(self.conv_norm_out(x, silu=True, **fk))  # conv_act (SiLU) fused into the norm
         out = x.reshape(b, f, x.shape[1], hh, ww).permute(0, 2, 1, 3, 4)
         return UNet3DConditionOutput(sample=out) if return_dict else (out,)

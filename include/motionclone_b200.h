@@ -111,6 +111,34 @@ int mc_cfg_ddim_step(const void* eps_cond, const void* eps_uncond, const void* x
                      int64_t n, float cfg_scale, float sqrt_beta_t, float inv_sqrt_alpha_t, float sqrt_alpha_prev,
                      float dir_coef, float score_coef, void* stream);
 
+/*
+ * The whole of customized_step (utils/motionclone_functions.py:339-404) behind the same CFG combine, still one pass and
+ * still the eager fp16 rounding sequence op by op. mc_cfg_ddim_step is this call with prediction_type = epsilon,
+ * flags = 0, noise = pred_x0 = NULL. With e the (combined) model output:
+ *   epsilon      (:340-341)  x0 = h(h(x - h(sb*e)) * inv_sa);   pe = e
+ *   sample       (:343-344)  x0 = e;                            pe = h(h(x - h(sa*x0)) * inv_sb)
+ *   v_prediction (:346-347)  x0 = h(h(sa*x) - h(sb*e));         pe = h(h(sa*e) + h(sb*x))
+ *   MC_DDIM_CLIP_SAMPLE  (:358-360)  x0 = h(min(max(x0, -clip_range), clip_range)), NaN kept
+ *   MC_DDIM_REDERIVE_EPS (:369, use_clipped_model_output)       pe = h(h(x - h(sa*x0)) * inv_sb)
+ *   score != NULL (:382)     pe = h(pe - h(sc*score))
+ *   (:386, :389)             x_prev = h(h(sap*x0) + h(dir_coef*pe)),  dir_coef = sqrt(1 - a_prev - std_dev^2)
+ *   noise != NULL (:402-404) x_prev = h(x_prev + h(std_dev*noise)),   std_dev = eta * sqrt(variance) (:364-365)
+ * sa = sqrt(a_t), inv_sb = 1/sqrt(1-a_t) (fp32), the others as for mc_cfg_ddim_step. noise is the caller's
+ * variance_noise (the generator's own stream; nothing is drawn here). pred_x0, when not NULL, receives x0 after the clip
+ * (the reference's pred_original_sample). Returns without a launch: MC_E_UNSUPPORTED for a prediction_type or flag bit
+ * not listed here; MC_E_INVALID for std_dev != 0 with noise == NULL (a missing noise tensor is not eta = 0), for a
+ * clip_range that is negative or NaN, and for null / misaligned (16 B) pointers.
+ */
+#define MC_DDIM_PRED_EPSILON 0
+#define MC_DDIM_PRED_SAMPLE 1
+#define MC_DDIM_PRED_V 2
+#define MC_DDIM_CLIP_SAMPLE 1
+#define MC_DDIM_REDERIVE_EPS 2
+int mc_ddim_step_ex(const void* eps_cond, const void* eps_uncond, const void* x, const void* score, const void* noise,
+                    void* x_prev, void* pred_x0, int64_t n, int prediction_type, int flags, float cfg_scale,
+                    float sqrt_beta_t, float inv_sqrt_alpha_t, float sqrt_alpha_prev, float dir_coef, float score_coef,
+                    float sqrt_alpha_t, float inv_sqrt_beta_t, float clip_range, float std_dev, void* stream);
+
 /* add_noise, utils/motionclone_functions.py:19-23: out = h(h(sa*x0) + h(sb*noise)). */
 int mc_add_noise(const void* x0, const void* noise, void* out, int64_t n, float sqrt_alpha, float sqrt_one_minus_alpha,
                  void* stream);

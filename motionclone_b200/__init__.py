@@ -7,12 +7,15 @@ __all__ = ["build_pipeline"]
 
 
 def build_pipeline(unet_config: dict, infer_config: dict, device="cuda", dtype=None, weight_seed: int = 42,
-                   state_dict=None, controlnet_kwargs=None, controlnet_state_dict=None, use_cuda_graphs: bool = True):
+                   state_dict=None, controlnet_kwargs=None, controlnet_state_dict=None, use_cuda_graphs: bool = True,
+                   scheduler_kwargs=None):
     """UNet3D (synthetic or given weights) + DDIMScheduler + AnimationPipeline with the nine functions bound
     (what t2v_video_sample.py:36-73 does). `controlnet_kwargs` (configs/sparsectrl/*.yaml controlnet_additional_kwargs)
     adds a SparseCtrl built with from_unet as i2v_video_sample.py:41-59 does (synthetic weights: seed + 1).
     `use_cuda_graphs`: the no-grad UNet forwards of the sampling loop (the plain step's b=2 forward, the guided step's
-    unconditional forward) are captured once per shape and replayed (guidance._GraphedUNetForward)."""
+    unconditional forward) are captured once per shape and replayed (guidance._GraphedUNetForward).
+    `scheduler_kwargs` are the inference YAML's noise_scheduler_kwargs (DDIMScheduler arguments such as prediction_type,
+    clip_sample, clip_sample_range), laid over the shipped ones (synthetic.NOISE_SCHEDULER_KWARGS)."""
     import torch
 
     from .guidance import bind_motionclone
@@ -38,6 +41,7 @@ def build_pipeline(unet_config: dict, infer_config: dict, device="cuda", dtype=N
             load_synthetic_weights(controlnet, weight_seed + 1)
         controlnet = controlnet.to(device=device, dtype=dtype).to(memory_format=torch.channels_last).eval()
     unet = unet.to(device=device, dtype=dtype).to(memory_format=torch.channels_last).eval()
-    pipe = AnimationPipeline(unet=unet, scheduler=DDIMScheduler(**NOISE_SCHEDULER_KWARGS), controlnet=controlnet)
+    pipe = AnimationPipeline(unet=unet, scheduler=DDIMScheduler(**dict(NOISE_SCHEDULER_KWARGS, **(scheduler_kwargs or {}))),
+                             controlnet=controlnet)
     pipe.use_cuda_graphs = bool(use_cuda_graphs)
     return bind_motionclone(pipe, _Config(dict(infer_config)))

@@ -24,7 +24,7 @@ class MotionCloneKernelError(RuntimeError):
 _lib = None
 
 EXPORTS = ("mc_abi_version", "mc_last_error", "mc_launch_count", "mc_reset_launch_count", "mc_add_launch_count", "mc_temporal_attn_fwd",
-           "mc_temporal_attn_bwd", "mc_top1_rows", "mc_motion_loss_fwd", "mc_motion_loss_bwd", "mc_cfg_ddim_step",
+           "mc_temporal_attn_bwd", "mc_top1_rows", "mc_motion_loss_fwd", "mc_motion_loss_bwd", "mc_cfg_ddim_step", "mc_ddim_step_ex",
            "mc_add_noise", "mc_groupnorm_workspace_bytes", "mc_groupnorm_nhwc", "mc_layernorm", "mc_geglu", "mc_groupnorm_nhwc_stats", "mc_groupnorm_nhwc_bwd", "mc_layernorm_bwd",
            "mc_groupnorm_nhwc_batched", "mc_groupnorm_nhwc_bwd_batched", "mc_groupnorm_nhwc_pooled",
            "mc_groupnorm_nhwc_bwd_pooled",
@@ -62,6 +62,8 @@ def lib() -> ctypes.CDLL:
     L.mc_motion_loss_bwd.argtypes = [c_int, POINTER(P), POINTER(P), POINTER(c_int64), P, POINTER(P), P]
     L.mc_cfg_ddim_step.restype = c_int
     L.mc_cfg_ddim_step.argtypes = [P, P, P, P, P, c_int64] + [c_float] * 6 + [P]
+    L.mc_ddim_step_ex.restype = c_int
+    L.mc_ddim_step_ex.argtypes = [P, P, P, P, P, P, P, c_int64, c_int, c_int] + [c_float] * 10 + [P]
     L.mc_add_noise.restype = c_int
     L.mc_add_noise.argtypes = [P, P, P, c_int64, c_float, c_float, P]
     L.mc_groupnorm_workspace_bytes.restype = c_int64

@@ -1,7 +1,9 @@
 // Fused elementwise / reduction kernels of the guided step (sm_90a): CFG combine + score-guided DDIM update,
 // add_noise, stand-alone top-1, and the motion-guidance loss with its closed-form gradient.
 // All are HBM / launch-latency bound: 128-bit coalesced accesses, grid sized in multiples of the SM count.
+#include <array>
 #include <mutex>
+#include <utility>
 
 #include "mc_common.cuh"
 
@@ -22,14 +24,29 @@ __device__ __forceinline__ uint4 ldg_nc_128(const void* p) {
   return r;
 }
 
-// One element of utils/motionclone_functions.py:239 + :339-389 with every intermediate rounded to fp16, in the order
-// the eager ATen kernels round (each binary op: fp32 opmath, fp16 result).
+// One element of utils/motionclone_functions.py:239 + :339-404 with every intermediate rounded to fp16, in the order
+// the eager ATen kernels round (each binary op: fp32 opmath, fp16 result; h = round to fp16). The 0-dim fp32 CPU
+// operands stay fp32, and `tensor / cpu_scalar` multiplies by the fp32 reciprocal. Per branch of the reference:
+//   CFG combine (:239, only with eps_uncond):  e = h(ec + h(cfg * h(ec - eu)))
+//   epsilon      (:340-341)  x0 = h(h(x - h(sb*e)) * inv_sa);            pe = e
+//   sample       (:343-344)  x0 = e;                                     pe = h(h(x - h(sa*x0)) * inv_sb)
+//   v_prediction (:346-347)  x0 = h(h(sa*x) - h(sb*e));                  pe = h(h(sa*e) + h(sb*x))
+//   clip_sample  (:358-360)  x0 = h(min(max(x0, -r), r)) in fp32, NaN kept (clamp_scalar_kernel_impl)
+//   use_clipped_model_output (:369)                                      pe = h(h(x - h(sa*x0)) * inv_sb)
+//   score        (:382)      pe = h(pe - h(sc*g))
+//   direction and sum (:386, :389)  xp = h(h(sap*x0) + h(c*pe)),  c = sqrt(1 - a_prev - std^2)
+//   eta > 0      (:402-404)  xp = h(xp + h(std*noise))
+// sb=sqrt(1-a_t), sa=sqrt(a_t), inv_* their fp32 reciprocals, sap=sqrt(a_prev), sc=guidance_scale*sqrt(1-a_t).
 struct DdimCoef {
   float cfg, sb, inv_sa, sap, c, sc;
+  float sa, inv_sb, clip, std;  // read by the sample / v_prediction / clip / re-derive / noise variants only
 };
 
-__device__ __forceinline__ __half ddim_one(__half ec, __half eu, bool has_u, __half x, __half g, bool has_g,
-                                           const DdimCoef& k) {
+enum { kPredEpsilon = MC_DDIM_PRED_EPSILON, kPredSample = MC_DDIM_PRED_SAMPLE, kPredV = MC_DDIM_PRED_V };
+
+template <int PRED, bool CLIP, bool REDERIVE, bool NOISE>
+__device__ __forceinline__ __half ddim_one(__half ec, __half eu, bool has_u, __half x, __half g, bool has_g, __half nz,
+                                           const DdimCoef& k, __half& x0_out) {
   const float fec = __half2float(ec);
   float e = fec;  // eps already combined by the caller (customized_step API) when there is no uncond operand
   if (has_u) {
@@ -37,42 +54,80 @@ __device__ __forceinline__ __half ddim_one(__half ec, __half eu, bool has_u, __h
     const float m = round_half(k.cfg * d);                      // cfg * (...)
     e = round_half(fec + m);                                    // eps
   }
-  const float t1 = round_half(k.sb * e);                        // sqrt(1-a_t) * eps
-  const float t2 = round_half(__half2float(x) - t1);            // x - ...
-  const float x0 = round_half(t2 * k.inv_sa);                   // / sqrt(a_t)  (CUDA: * fp32 reciprocal)
-  float e2 = e;
+  float x0, e2;
+  if constexpr (PRED == kPredEpsilon) {
+    const float t1 = round_half(k.sb * e);                      // sqrt(1-a_t) * eps
+    const float t2 = round_half(__half2float(x) - t1);          // x - ...
+    x0 = round_half(t2 * k.inv_sa);                             // / sqrt(a_t)  (CUDA: * fp32 reciprocal)
+    e2 = e;
+  } else if constexpr (PRED == kPredSample) {
+    x0 = e;
+    const float t1 = round_half(k.sa * x0);                     // sqrt(a_t) * x0
+    const float t2 = round_half(__half2float(x) - t1);
+    e2 = round_half(t2 * k.inv_sb);                             // / sqrt(1-a_t)
+  } else {
+    const float xf = __half2float(x);
+    x0 = round_half(round_half(k.sa * xf) - round_half(k.sb * e));
+    e2 = round_half(round_half(k.sa * e) + round_half(k.sb * xf));
+  }
+  if constexpr (CLIP) {
+    if (x0 == x0) x0 = round_half(fminf(fmaxf(x0, -k.clip), k.clip));
+  }
+  if constexpr (REDERIVE) {
+    const float t1 = round_half(k.sa * x0);
+    const float t2 = round_half(__half2float(x) - t1);
+    e2 = round_half(t2 * k.inv_sb);
+  }
   if (has_g) {
     const float g2 = round_half(k.sc * __half2float(g));        // guidance_scale*sqrt(1-a_t) * score
-    e2 = round_half(e - g2);
+    e2 = round_half(e2 - g2);
   }
-  const float dir = round_half(k.c * e2);                       // sqrt(1-a_prev) * eps'
+  const float dir = round_half(k.c * e2);                       // sqrt(1-a_prev-std^2) * eps'
   const float t3 = round_half(k.sap * x0);                      // sqrt(a_prev) * x0
+  x0_out = __float2half_rn(x0);
+  if constexpr (NOISE) {
+    const float xp = round_half(t3 + dir);
+    return __float2half_rn(xp + round_half(k.std * __half2float(nz)));  // + std * variance_noise
+  }
   return __float2half_rn(t3 + dir);
 }
 
+// <epsilon, no clip, no re-derive, no noise, no x0 store> is the guided sampling loop's step; the other instantiations
+// add only what their branch needs (noise: a fifth 128-bit load; WRITE_X0: a second 128-bit store of pred_original_sample).
+template <int PRED, bool CLIP, bool REDERIVE, bool NOISE, bool WRITE_X0>
 __global__ void __launch_bounds__(256) cfg_ddim_step_kernel(const __half* __restrict__ ec, const __half* __restrict__ eu,
                                                             const __half* __restrict__ x,
                                                             const __half* __restrict__ score, __half* __restrict__ out,
-                                                            int64_t n, DdimCoef k) {
+                                                            int64_t n, DdimCoef k, const __half* __restrict__ noise,
+                                                            __half* __restrict__ x0_out) {
   const int64_t nvec = n / 8;
   const bool has_g = score != nullptr;
   const bool has_u = eu != nullptr;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nvec; i += (int64_t)gridDim.x * blockDim.x) {
-    Pack8 a, b, c, d, o;
+    Pack8 a, b, c, d, z, o, p;
     a.u = ldg_nc_128(ec + i * 8);
     if (has_u) b.u = ldg_nc_128(eu + i * 8);
     c.u = ldg_nc_128(x + i * 8);
     if (has_g) d.u = ldg_nc_128(score + i * 8);
+    if constexpr (NOISE) z.u = ldg_nc_128(noise + i * 8);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      o.h[j] = ddim_one(a.h[j], has_u ? b.h[j] : __half(), has_u, c.h[j], has_g ? d.h[j] : __half(), has_g, k);
+      o.h[j] = ddim_one<PRED, CLIP, REDERIVE, NOISE>(a.h[j], has_u ? b.h[j] : __half(), has_u, c.h[j],
+                                                     has_g ? d.h[j] : __half(), has_g, NOISE ? z.h[j] : __half(), k,
+                                                     p.h[j]);
     *reinterpret_cast<uint4*>(out + i * 8) = o.u;
+    if constexpr (WRITE_X0) *reinterpret_cast<uint4*>(x0_out + i * 8) = p.u;
   }
   // tail (n % 8), one thread each
   const int64_t tail0 = nvec * 8;
   const int64_t ti = tail0 + blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (ti < n)
-    out[ti] = ddim_one(ec[ti], has_u ? eu[ti] : __half(), has_u, x[ti], has_g ? score[ti] : __half(), has_g, k);
+  if (ti < n) {
+    __half p;
+    out[ti] = ddim_one<PRED, CLIP, REDERIVE, NOISE>(ec[ti], has_u ? eu[ti] : __half(), has_u, x[ti],
+                                                    has_g ? score[ti] : __half(), has_g, NOISE ? noise[ti] : __half(), k,
+                                                    p);
+    if constexpr (WRITE_X0) x0_out[ti] = p;
+  }
 }
 
 __global__ void __launch_bounds__(256) add_noise_kernel(const __half* __restrict__ x0, const __half* __restrict__ nz,
@@ -257,24 +312,76 @@ static unsigned grid_for(int64_t nvec, int threads) {
 
 }  // namespace mc
 
+using DdimStepKernel = void (*)(const __half*, const __half*, const __half*, const __half*, __half*, int64_t,
+                                mc::DdimCoef, const __half*, __half*);
+
+// row PRED of the variant table; column bits: 1 clip, 2 re-derive, 4 noise, 8 x0 store
+template <int PRED, size_t... V>
+static constexpr std::array<DdimStepKernel, sizeof...(V)> ddim_step_row(std::index_sequence<V...>) {
+  return {mc::cfg_ddim_step_kernel<PRED, (V & 1) != 0, (V & 2) != 0, (V & 4) != 0, (V & 8) != 0>...};
+}
+
+static int launch_ddim_step(const char* what, int pred, unsigned variant, const void* eps_cond, const void* eps_uncond,
+                            const void* x, const void* score, const void* noise, void* x_prev, void* pred_x0, int64_t n,
+                            const mc::DdimCoef& k, void* stream) {
+  using namespace mc;
+  static constexpr std::array<DdimStepKernel, 16> table[3] = {
+      ddim_step_row<kPredEpsilon>(std::make_index_sequence<16>()),
+      ddim_step_row<kPredSample>(std::make_index_sequence<16>()),
+      ddim_step_row<kPredV>(std::make_index_sequence<16>())};
+  if (!eps_cond || !x || !x_prev || n <= 0) {
+    set_error("%s: null pointer or n <= 0", what);
+    return MC_E_INVALID;
+  }
+  const uintptr_t al = (uintptr_t)eps_cond | (uintptr_t)eps_uncond | (uintptr_t)x | (uintptr_t)x_prev |
+                       (uintptr_t)score | (uintptr_t)noise | (uintptr_t)pred_x0;
+  if (al & 15) {
+    set_error("%s: pointers must be 16-byte aligned", what);
+    return MC_E_INVALID;
+  }
+  table[pred][variant]<<<grid_for(n / 8 + 8, 256), 256, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_cond, (const __half*)eps_uncond, (const __half*)x, (const __half*)score, (__half*)x_prev, n, k,
+      (const __half*)noise, (__half*)pred_x0);
+  count_launch();
+  return check_launch(what);
+}
+
 extern "C" int mc_cfg_ddim_step(const void* eps_cond, const void* eps_uncond, const void* x, const void* score,
                                 void* x_prev, int64_t n, float cfg_scale, float sqrt_beta_t, float inv_sqrt_alpha_t,
                                 float sqrt_alpha_prev, float dir_coef, float score_coef, void* stream) {
+  mc::DdimCoef k{cfg_scale, sqrt_beta_t, inv_sqrt_alpha_t, sqrt_alpha_prev, dir_coef, score_coef, 0.f, 0.f, 0.f, 0.f};
+  return launch_ddim_step("cfg_ddim_step", MC_DDIM_PRED_EPSILON, 0u, eps_cond, eps_uncond, x, score, nullptr, x_prev,
+                          nullptr, n, k, stream);
+}
+
+extern "C" int mc_ddim_step_ex(const void* eps_cond, const void* eps_uncond, const void* x, const void* score,
+                               const void* noise, void* x_prev, void* pred_x0, int64_t n, int prediction_type, int flags,
+                               float cfg_scale, float sqrt_beta_t, float inv_sqrt_alpha_t, float sqrt_alpha_prev,
+                               float dir_coef, float score_coef, float sqrt_alpha_t, float inv_sqrt_beta_t,
+                               float clip_range, float std_dev, void* stream) {
   using namespace mc;
-  if (!eps_cond || !x || !x_prev || n <= 0) {
-    set_error("cfg_ddim_step: null pointer or n <= 0");
+  if (prediction_type < MC_DDIM_PRED_EPSILON || prediction_type > MC_DDIM_PRED_V) {
+    set_error("ddim_step_ex: prediction_type=%d is not epsilon (0), sample (1) or v_prediction (2)", prediction_type);
+    return MC_E_UNSUPPORTED;
+  }
+  if (flags & ~(MC_DDIM_CLIP_SAMPLE | MC_DDIM_REDERIVE_EPS)) {
+    set_error("ddim_step_ex: unknown flag bits 0x%x", (unsigned)flags);
+    return MC_E_UNSUPPORTED;
+  }
+  if ((flags & MC_DDIM_CLIP_SAMPLE) && !(clip_range >= 0.f)) {
+    set_error("ddim_step_ex: clip_range must be >= 0 with MC_DDIM_CLIP_SAMPLE");
     return MC_E_INVALID;
   }
-  const uintptr_t al = (uintptr_t)eps_cond | (uintptr_t)eps_uncond | (uintptr_t)x | (uintptr_t)x_prev | (uintptr_t)score;
-  if (al & 15) {
-    set_error("cfg_ddim_step: pointers must be 16-byte aligned");
+  if (!noise && std_dev != 0.f) {
+    set_error("ddim_step_ex: std_dev=%g needs a noise tensor (NULL noise is not eta = 0)", (double)std_dev);
     return MC_E_INVALID;
   }
-  DdimCoef k{cfg_scale, sqrt_beta_t, inv_sqrt_alpha_t, sqrt_alpha_prev, dir_coef, score_coef};
-  cfg_ddim_step_kernel<<<grid_for(n / 8 + 8, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const __half*)eps_cond, (const __half*)eps_uncond, (const __half*)x, (const __half*)score, (__half*)x_prev, n, k);
-  count_launch();
-  return check_launch("cfg_ddim_step");
+  const unsigned variant = ((flags & MC_DDIM_CLIP_SAMPLE) ? 1u : 0u) | ((flags & MC_DDIM_REDERIVE_EPS) ? 2u : 0u) |
+                           (noise ? 4u : 0u) | (pred_x0 ? 8u : 0u);
+  DdimCoef k{cfg_scale, sqrt_beta_t, inv_sqrt_alpha_t, sqrt_alpha_prev, dir_coef, score_coef,
+             sqrt_alpha_t, inv_sqrt_beta_t, clip_range, std_dev};
+  return launch_ddim_step("ddim_step_ex", prediction_type, variant, eps_cond, eps_uncond, x, score, noise, x_prev, pred_x0,
+                          n, k, stream);
 }
 
 extern "C" int mc_add_noise(const void* x0, const void* noise, void* out, int64_t n, float sqrt_alpha,

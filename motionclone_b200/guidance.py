@@ -494,17 +494,75 @@ def _step_alphas(self, step_index):
     return a_t, a_prev
 
 
-def _check_step_args(self, eta, use_clipped_model_output, variance_noise, indices, return_middle):
+def _check_step_args(self, indices, return_middle):
     if self.num_inference_steps is None:
         raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
                          "scheduler")  # :303-306
     pt = self.config.prediction_type
-    if pt not in ("epsilon", "sample", "v_prediction"):
+    if pt not in ops.PREDICTION_TYPES:  # :348-352
         raise ValueError(f"prediction_type given as {pt} must be one of `epsilon`, `sample`, or `v_prediction`")
-    if pt != "epsilon" or self.config.thresholding or self.config.clip_sample or eta != 0.0 \
-            or use_clipped_model_output or variance_noise is not None or indices is not None or return_middle:
-        raise NotImplementedError("only the live configuration is built: epsilon prediction, eta=0, no clip/threshold, "
-                                  "no indices/return_middle (SURVEY.md appendix A)")
+    unbuilt = [name for name, on in (("thresholding", self.config.thresholding), ("indices", indices is not None),
+                                     ("return_middle", return_middle),
+                                     ("learned variance", self.variance_type in ("learned", "learned_range"))) if on]
+    if unbuilt:
+        raise NotImplementedError(f"customized_step: {', '.join(unbuilt)} not built (dynamic thresholding is a per-sample "
+                                  "quantile, a kernel of its own; the others are dead in every shipped config, "
+                                  "SURVEY.md appendix A)")
+
+
+def randn_tensor(shape, generator=None, device=None, dtype=None):
+    """diffusers 0.16 utils.randn_tensor: a CPU generator draws on the CPU and the result is moved to `device`, a
+    generator of the device draws there; a list of B generators draws one [1, ...] tensor each and concatenates, so
+    sample s of a batch gets the noise its own generator gives in a B = 1 call."""
+    device = torch.device(device)
+    rand_device = device
+    batch_size = shape[0]
+    if generator is not None:
+        gen_type = (generator[0] if isinstance(generator, (list, tuple)) else generator).device.type
+        if gen_type != device.type and gen_type == "cpu":
+            rand_device = torch.device("cpu")
+        elif gen_type != device.type and gen_type == "cuda":
+            raise ValueError(f"Cannot generate a {device} tensor from a generator of type {gen_type}.")
+    if isinstance(generator, (list, tuple)):
+        if len(generator) != batch_size:
+            raise ValueError(f"{len(generator)} generators for a batch of {batch_size}")
+        one = (1,) + tuple(shape[1:])
+        return torch.cat([torch.randn(one, generator=g, device=rand_device, dtype=dtype) for g in generator],
+                         dim=0).to(device)
+    return torch.randn(tuple(shape), generator=generator, device=rand_device, dtype=dtype).to(device)
+
+
+def _variance_noise(model_output, eta, generator, variance_noise):
+    """:391-401. Nothing is drawn when eta <= 0: the generator's state is untouched."""
+    if not eta > 0:
+        return None
+    if variance_noise is not None and generator is not None:
+        raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either `generator` or"
+                         " `variance_noise` stays `None`.")
+    if variance_noise is None:
+        return randn_tensor(model_output.shape, generator=generator, device=model_output.device,
+                            dtype=model_output.dtype)
+    return variance_noise.to(device=model_output.device, dtype=model_output.dtype)
+
+
+def _fused_step(self, eps_cond, eps_uncond, cfg_scale, step_index, sample, score, guidance_scale, eta,
+                use_clipped_model_output, generator, variance_noise, want_pred_x0):
+    """One launch for CFG combine + :339-404. The variant follows from the scheduler's configuration and the step's
+    arguments alone; the configuration the guided loop ships with (epsilon, no clip, eta = 0) takes mc_cfg_ddim_step."""
+    a_t, a_prev = _step_alphas(self, step_index)
+    if score is not None:
+        assert eps_cond.shape == score.shape  # :381
+    if score is None or not guidance_scale > 0.0:
+        score = None
+    cfg = self.config
+    noise = _variance_noise(eps_cond, eta, generator, variance_noise)
+    if cfg.prediction_type == "epsilon" and not cfg.clip_sample and not use_clipped_model_output and eta == 0.0:
+        return ops.cfg_ddim_step(eps_cond, eps_uncond, sample, score, cfg_scale, a_t, a_prev, guidance_scale), None, a_prev
+    prev_sample, pred_x0 = ops.ddim_step(
+        eps_cond, eps_uncond, sample, score, cfg_scale, a_t, a_prev, guidance_scale, prediction_type=cfg.prediction_type,
+        clip_sample_range=cfg.clip_sample_range if cfg.clip_sample else None,
+        use_clipped_model_output=bool(use_clipped_model_output), eta=eta, noise=noise, want_pred_x0=want_pred_x0)
+    return prev_sample, pred_x0, a_prev
 
 
 @torch.no_grad()
@@ -512,28 +570,27 @@ def schedule_customized_step(self, model_output, step_index: int, sample, eta: f
                              use_clipped_model_output: bool = False, generator=None, variance_noise=None,
                              return_dict: bool = True, score=None, guidance_scale=1.0, indices=None,
                              return_middle=False):
-    """:285-409 (`model_output` is the already CFG-combined epsilon, as the reference calls it at :241/:256)."""
-    _check_step_args(self, eta, use_clipped_model_output, variance_noise, indices, return_middle)
-    a_t, a_prev = _step_alphas(self, step_index)
-    if score is not None:
-        assert model_output.shape == score.shape  # :381
-    use_score = score is not None and guidance_scale > 0.0
-    prev_sample = ops.cfg_ddim_step(model_output, None, sample, score if use_score else None, 0.0, a_t, a_prev,
-                                    guidance_scale)
+    """:285-409 (`model_output` is the already CFG-combined model output, as the reference calls it at :241/:256): every
+    `prediction_type`, `clip_sample` / `clip_sample_range`, `use_clipped_model_output`, and eta > 0 with the noise of
+    `generator` (one, or a list of B for a batch of B) or `variance_noise`. Returns the reference's tuple
+    (prev_sample, pred_original_sample, alpha_prod_t_prev); on the shipped configuration (epsilon prediction, no clip,
+    eta = 0, `use_clipped_model_output=False`) pred_original_sample is None, as it is not part of that launch."""
+    _check_step_args(self, indices, return_middle)
+    out = _fused_step(self, model_output, None, 0.0, step_index, sample, score, guidance_scale, eta,
+                      use_clipped_model_output, generator, variance_noise, want_pred_x0=return_dict)
     if not return_dict:
-        return (prev_sample,)
-    return prev_sample, None, a_prev
+        return (out[0],)
+    return out
 
 
 @torch.no_grad()
 def schedule_customized_step_fused(self, eps_cond, eps_uncond, cfg_scale: float, step_index: int, sample,
-                                   score=None, guidance_scale=1.0, eta: float = 0.0, generator=None):
-    """CFG combine (:239/:255) + customized_step (:285-409) in ONE launch; returns x_{t-1}."""
-    _check_step_args(self, eta, False, None, None, False)
-    a_t, a_prev = _step_alphas(self, step_index)
-    use_score = score is not None and guidance_scale > 0.0
-    return ops.cfg_ddim_step(eps_cond, eps_uncond, sample, score if use_score else None, cfg_scale, a_t, a_prev,
-                             guidance_scale)
+                                   score=None, guidance_scale=1.0, eta: float = 0.0, generator=None,
+                                   variance_noise=None, use_clipped_model_output: bool = False):
+    """CFG combine (:239/:255) + customized_step (:285-409) in ONE launch for the whole batch; returns x_{t-1}."""
+    _check_step_args(self, None, False)
+    return _fused_step(self, eps_cond, eps_uncond, cfg_scale, step_index, sample, score, guidance_scale, eta,
+                       use_clipped_model_output, generator, variance_noise, want_pred_x0=False)[0]
 
 
 def schedule_set_timesteps(self, num_inference_steps: int, guidance_steps: int = 0, guiduance_scale: float = 0.0,

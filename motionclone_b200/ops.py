@@ -301,6 +301,56 @@ def cfg_ddim_step(eps_cond: Tensor, eps_uncond: Optional[Tensor], x: Tensor, sco
     return out
 
 
+PREDICTION_TYPES = {"epsilon": 0, "sample": 1, "v_prediction": 2}  # MC_DDIM_PRED_*
+
+
+def ddim_std_dev(alpha_t: Tensor, alpha_prev: Tensor, eta: float) -> Tensor:
+    """std_dev_t of motionclone_functions.py:364-365 (diffusers 0.16 DDIMScheduler._get_variance) as a 0-dim fp32 CPU
+    tensor, in the reference's fp32 op order."""
+    a_t = alpha_t.detach().to(torch.float32).cpu()
+    a_p = alpha_prev.detach().to(torch.float32).cpu()
+    variance = ((1 - a_p) / (1 - a_t)) * (1 - a_t / a_p)
+    return eta * variance ** 0.5
+
+
+def ddim_step(eps_cond: Tensor, eps_uncond: Optional[Tensor], x: Tensor, score: Optional[Tensor], cfg_scale: float,
+              alpha_t: Tensor, alpha_prev: Tensor, guidance_scale: float = 1.0, *, prediction_type: str = "epsilon",
+              clip_sample_range: Optional[float] = None, use_clipped_model_output: bool = False, eta: float = 0.0,
+              noise: Optional[Tensor] = None, want_pred_x0: bool = False):
+    """One fused launch for motionclone_functions.py:239 + the whole of :339-404 (mc_ddim_step_ex): the three prediction
+    types, x0 clipping to +-`clip_sample_range` (None: no clip), epsilon re-derived from the clipped x0, score guidance and
+    the stochastic term std_dev_t * `noise` of eta > 0. `noise` is the variance noise of :398-401 and is required exactly
+    when eta > 0 (it is read even where std_dev_t is 0, as the reference adds it there). Scalars as in `cfg_ddim_step`.
+    Returns (x_prev, pred_original_sample or None)."""
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample`, or "
+                         "`v_prediction`")
+    if (eta > 0) != (noise is not None):
+        raise ValueError("ddim_step: `noise` must be given exactly when eta > 0")
+    tensors = {"eps_cond": eps_cond, "x": x, "eps_uncond": eps_uncond, "score": score, "noise": noise}
+    for name, t in tensors.items():
+        if t is not None:
+            _require(t, name)
+            if t.shape != x.shape:
+                raise ValueError(f"ddim_step: {name} has shape {tuple(t.shape)}, x has {tuple(x.shape)}")
+            tensors[name] = t.contiguous()
+    eps_cond, x, eps_uncond, score, noise = (tensors[k] for k in ("eps_cond", "x", "eps_uncond", "score", "noise"))
+    a_t = alpha_t.detach().to(torch.float32).cpu()
+    a_p = alpha_prev.detach().to(torch.float32).cpu()
+    std = ddim_std_dev(a_t, a_p, eta)
+    sa, sb = a_t ** 0.5, (1 - a_t) ** 0.5
+    flags = (1 if clip_sample_range is not None else 0) | (2 if use_clipped_model_output else 0)
+    out = torch.empty_like(x)
+    pred_x0 = torch.empty_like(x) if want_pred_x0 else None
+    st = _lib.lib().mc_ddim_step_ex(_ptr(eps_cond), _ptr(eps_uncond), _ptr(x), _ptr(score), _ptr(noise), _ptr(out),
+                                    _ptr(pred_x0), x.numel(), PREDICTION_TYPES[prediction_type], flags, float(cfg_scale),
+                                    float(sb), float(1.0 / sa), float(a_p ** 0.5), float((1 - a_p - std ** 2) ** 0.5),
+                                    float(guidance_scale * (1 - a_t) ** 0.5), float(sa), float(1.0 / sb),
+                                    float(clip_sample_range or 0.0), float(std), _stream())
+    _lib.check(st, "mc_ddim_step_ex")
+    return out, pred_x0
+
+
 def add_noise(x0: Tensor, noise: Tensor, alpha_t: Tensor) -> Tensor:
     """motionclone_functions.py:19-23."""
     _require(x0, "x0"), _require(noise, "noise")

@@ -90,7 +90,9 @@ int mc_top1_rows(const void* probs, int64_t rows, int L, void* top_val, uint8_t*
 /*
  * Motion-guidance loss (utils/motionclone_functions.py:85-100) on gathered probabilities:
  *   loss_per_module[m] = fp16( mean_i fp16(fp16(cur_m[i] - ref_m[i])^2) ),  loss_total = fp16(sum_m loss_per_module[m])
- * (the rounding sequence of F.mse_loss on half tensors followed by stack().sum()). M <= 16 modules.
+ * (the rounding sequence of F.mse_loss on half tensors followed by stack().sum()). 1 <= M <= 64 modules (all 40
+ * temporal attentions of an SD1.5 UNet, plus 2 for a mid-block motion module); any other M returns MC_E_INVALID
+ * without a launch. One CTA per module and the module-order total keep the result of a call independent of the cap.
  */
 int mc_motion_loss_fwd(int M, const void* const* cur, const void* const* ref, const int64_t* n,
                        void* loss_per_module, void* loss_total, void* stream);

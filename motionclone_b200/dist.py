@@ -2,8 +2,9 @@
 
 The reference is single-process / single-GPU (SURVEY.md §2a). Samples (JSONL lines, t2v_video_sample.py:75-105) are
 independent, so the path shards with no data-path collective; the only shared state is the reference clip's motion
-representation (6 x (fp16 values + uint8 indices), 590 KB at 16x512x512), which rank 0 extracts once and broadcasts
-as a single contiguous byte buffer (NCCL on GPUs, gloo in the CPU tests)."""
+representation (6 x (fp16 values + uint8 indices), 590 KB at 16x512x512 for the shipped `up_blocks.1`), which rank 0
+extracts once and broadcasts as a single contiguous byte buffer (NCCL on GPUs, gloo in the CPU tests). Guided modules
+at other or mixed UNet levels have sizes of their own: `representation_manifest_for` derives them from the UNet."""
 from __future__ import annotations
 
 import os
@@ -61,6 +62,32 @@ def representation_manifest(module_names: Sequence[str], positions: int, heads: 
     ONLY collective of the path."""
     shape = (int(positions), int(heads), int(frames), 1)
     return [(str(n), shape, shape) for n in module_names]
+
+
+def representation_manifest_for(unet, module_names: Sequence[str], height: int, width: int, frames: int) -> list:
+    """The manifest for guided modules at any UNet level (any `motion_guidance_blocks`): module m gets
+    [positions_m, heads_m, frames, 1], positions_m the latent positions at m's level. Level 0 is the latent
+    (height / 8) x (width / 8); each down block but the last halves it, rounding up (stride-2 conv, padding 1);
+    down_blocks.i runs at level i, the mid block at the last level and up_blocks.i at level (levels - 1 - i)."""
+    levels = len(unet.down_blocks)
+    sizes = [(int(height) // 8, int(width) // 8)]
+    for _ in range(levels - 1):
+        sizes.append(((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2))
+    out = []
+    for name in module_names:
+        parts = str(name).split(".")
+        if parts[0] == "down_blocks":
+            level = int(parts[1])
+        elif parts[0] == "up_blocks":
+            level = levels - 1 - int(parts[1])
+        elif parts[0] == "mid_block":
+            level = levels - 1
+        else:
+            raise ValueError(f"'{name}' is not a module of the down, mid or up blocks")
+        h, w = sizes[level]
+        shape = (h * w, int(unet.get_submodule(str(name)).heads), int(frames), 1)
+        out.append((str(name), shape, shape))
+    return out
 
 
 def manifest_nbytes(manifest: list) -> int:

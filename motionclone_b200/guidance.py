@@ -63,6 +63,16 @@ def guided_modules(self) -> Dict[str, VersatileAttention]:
             if "VersatileAttention" in type(m).__name__ and classify_blocks(blocks, name)}
 
 
+def _guidance_layout(self):
+    """(cut, guided module names, the guided modules in up blocks after the cut). Down-block and mid-block modules and
+    those in up blocks <= cut run under grad in the conditional pass and before extraction's early return
+    (motionclone_functions.py:602, :627-629); the others run under no_grad, and extraction never reaches them."""
+    cut = self.unet._guidance_cut()
+    names = list(guided_modules(self))
+    late = [n for n in names if n.startswith("up_blocks.") and int(n.split(".")[1]) > cut]
+    return cut, names, late
+
+
 def _set_processor_mode(self, mode: Optional[str], ref_idx: Optional[Dict[str, torch.Tensor]] = None):
     for name, m in guided_modules(self).items():
         if m.processor is None:
@@ -114,6 +124,12 @@ def obtain_motion_representation(self, generator=None, motion_representation_pat
     latents, BASELINE.json configs); decoding a video file + VAE + CLIP are outside the path (SURVEY.md §2 #9, #12)
     and require `self.vae` / `self.text_encoder` objects supplied by the caller."""
     cfg = self.input_config
+    cut, _, late = _guidance_layout(self)
+    if late:
+        raise ValueError(f"motion_guidance_blocks: guided module(s) {late} lie in up blocks after the cut up_blocks.{cut} "
+                         f"(the suffix of the last entry, {list(_cfg_get(cfg, 'motion_guidance_blocks'))[-1]!r}); "
+                         "extraction stops after that block and never runs them. End the list with the highest guided "
+                         "up block.")
     video_latents = _cfg_get(cfg, "video_latents")
     if video_latents is None:
         raise NotImplementedError("video decode + VAE encode are outside the hot path: pass input_config.video_latents")
@@ -163,7 +179,8 @@ def obtain_motion_representation(self, generator=None, motion_representation_pat
 # ----------------------------------------------------------------------------------------------------------------
 def _check_representation(rep, frames: int, label: str = "motion representation"):
     """Value / index tensors of shape [N, heads, frames, 1] with every index < frames (a stale or foreign .pt must fail
-    here, as torch.gather would at :91-92)."""
+    here, as torch.gather would at :91-92). N is checked per module, so modules of different UNet levels (N = the
+    latent positions of the module's level) are accepted side by side."""
     for k, (val, idx) in rep.items():
         if val.shape != idx.shape or val.dim() != 4 or val.shape[-1] != 1:
             raise ValueError(f"{label} '{k}': expected value / index tensors of shape [N, heads, L, 1], "
@@ -328,6 +345,11 @@ def sample_video(self, eta: float = 0.0, generator=None, noisy_latents: Optional
     if 2 * batch_size * frames > 1024:  # the plain step's b = 2B UNet pass: GroupNorm takes at most 1024 frames
         raise ValueError(f"a batch of {batch_size} x {frames} frames exceeds 1024 frames in the b = 2B UNet pass: "
                          f"use at most {1024 // (2 * frames)} samples per call")
+    cut, names, late = _guidance_layout(self)
+    if _cfg_get(cfg, "guidance_steps") > 0 and len(late) == len(names):
+        raise ValueError(f"motion_guidance_blocks {list(_cfg_get(cfg, 'motion_guidance_blocks'))}: no guided module "
+                         f"runs under grad (guided: {names}; the cut is up_blocks.{cut}, and later up blocks run under "
+                         "no_grad), so the guidance loss has no gradient")
     reps = _resolve_representations(self, motion_representation, batch_size, frames)
     self.add_controlnet = add_controlnet
     if add_controlnet:  # :111-128 — image files + VAE encode are off the path: the caller passes their result

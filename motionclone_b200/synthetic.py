@@ -44,6 +44,9 @@ UNET_TINY_CONFIG = dict(UNET_SD15_CONFIG, sample_size=16, block_out_channels=(64
 UNET_SD15_POOLED_GN_CONFIG = dict(UNET_SD15_CONFIG, use_inflated_groupnorm=False)
 UNET_TINY_POOLED_GN_CONFIG = dict(UNET_TINY_CONFIG, use_inflated_groupnorm=False)
 
+# configs/model_config/inference-v2.yaml: a motion module in the mid block as well (two more temporal attentions)
+UNET_TINY_MIDV2_CONFIG = dict(UNET_TINY_CONFIG, motion_module_mid_block=True)
+
 # configs/model_config/model_config.yaml:17-21
 NOISE_SCHEDULER_KWARGS = dict(beta_start=0.00085, beta_end=0.012, beta_schedule="linear", steps_offset=1,
                               clip_sample=False)

@@ -473,7 +473,10 @@ class UNet3DConditionModel(nn.Module):
         if isinstance(attention_head_dim, int):
             attention_head_dim = (attention_head_dim,) * len(down_block_types)
 
+        # registered before the mid block, as in unet.py:116-118 (`self.mid_block = None` registers nothing): module
+        # order down, up, mid is the key order of a motion representation that guides the mid block's motion module
         self.down_blocks = nn.ModuleList()
+        self.up_blocks = nn.ModuleList()
         out_c = ch[0]
         for i, btype in enumerate(down_block_types):
             res = 2 ** i
@@ -497,7 +500,6 @@ class UNet3DConditionModel(nn.Module):
             motion_module_kwargs=motion_module_kwargs, use_inflated_groupnorm=use_inflated_groupnorm)
 
         self.num_upsamplers = 0
-        self.up_blocks = nn.ModuleList()
         rch = list(reversed(ch))
         rheads = list(reversed(attention_head_dim))
         out_c = rch[0]
@@ -542,6 +544,9 @@ class UNet3DConditionModel(nn.Module):
 
     # ---- forward ----
     def _guidance_cut(self) -> int:
+        """Index of the last up block that runs under grad (and, in extraction, at all): the integer suffix of the last
+        `motion_guidance_blocks` entry (motionclone_functions.py:602). An entry without one ('mid_block', 'up_blocks')
+        raises the ValueError of int(), as in the reference."""
         cfg = self.input_config
         blocks = getattr(cfg, "motion_guidance_blocks", None) if cfg is not None else None
         if blocks is None and isinstance(cfg, dict):
@@ -560,6 +565,7 @@ class UNet3DConditionModel(nn.Module):
         encoder_hidden_states `[b, 77, c]`; returns `.sample [b, 4, f, h, w]`."""
         if attention_mask is not None or class_labels is not None:
             raise NotImplementedError("attention_mask / class_labels are never passed on the live path")
+        cut = self._guidance_cut()  # before any launch: a bad block list fails here, not after the down blocks ran
         b, cin, f, hh, ww = sample.shape
         up_factor = 2 ** self.num_upsamplers
         forward_upsample_size = any(s % up_factor != 0 for s in (hh, ww))  # :516-518
@@ -592,7 +598,6 @@ class UNet3DConditionModel(nn.Module):
         if mid_block_additional_residual is not None:
             x = x + as4d(mid_block_additional_residual)
 
-        cut = self._guidance_cut()
         for i, blk in enumerate(self.up_blocks):
             if i > cut and only_motion_feature:
                 return 0  # :627-628
